@@ -2,6 +2,7 @@
 """Benchmark of the multi-view denoising hot path (BASELINE.json: "6-view 224x400 denoising-steps/sec").
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload full|cam] [--scenes S]
+                  [--dump-outputs DIR]
 
 One "step" = ControlNet forward + multi-view UNet forward + classifier-free-guidance combine + DDIM update for S
 six-view scenes per GPU (CFG on: 12 view-samples per scene-step, the reference default guidance_scale = 2).
@@ -55,6 +56,10 @@ def parse():
                     help="N>1: scenes = independent scenes per GPU (default, weak scaling, no data-path collective); "
                          "views = the 6 cameras of the SAME scenes split across GPUs with an exchange of the "
                          "cross-view K/V per multiview block (strong scaling, latency mode)")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="after the timed steps, write the latents the last timed step produced (what a caller of the denoising "
+                         "step receives) as DIR/latents.npy, float32 [scenes, views, 4, h, w]; inputs are seeded, so two builds "
+                         "run with the same arguments can be compared output for output")
     ap.add_argument("--strong-scaling", action="store_true",
                     help="N>1, default sharding: after the replica measurement also time ONE scene spread over all N GPUs "
                          "(guidance halves x views through NVLink peer memory) and report it as `strong_scaling`")
@@ -79,11 +84,11 @@ def workload_config(args, sharding):
                         + ", CFG 2.0 (12 view-samples per scene-step), DDIM eta=0, SD-1.5-config UNet + BEVControlNet, random-init weights",
             "scenes_per_gpu": args.scenes, "views": 6, "latent_hw": [28, 50] if args.res == "224x400" else [53, 100],
             "sharding": sharding, "scheduler": args.scheduler,
-            "l2": "2.6 GB of weights are streamed every step (>> 126 MB L2), no explicit flush needed"}
+            "l2": "2.6 GB of weights are streamed every step (>> 50 MB L2), no explicit flush needed"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, index):
         self.index, self.rows, self.proc = index, [], None
@@ -140,8 +145,8 @@ def calibrate_cpu_threads():
 
 class ReferenceArm:
     """The reference's own implementation of the path on this workload (oracle/ref_runner.py: the unmodified
-    StableDiffusionBEVControlNetPipeline.__call__ with its own networks), or — if neither /root/reference nor the
-    oracle/_ref snapshot exists — the oracle port (oracle/torch_oracle.py).  Measurement code only."""
+    StableDiffusionBEVControlNetPipeline.__call__ with its own networks), or — if neither the reference tree nor the
+    oracle/_ref snapshot is available — the oracle port (oracle/torch_oracle.py).  Measurement code only."""
 
     def __init__(self, args):
         from oracle import ref_runner
@@ -336,6 +341,12 @@ def main():
         ms_total = tt.item()
     ms_step = ms_total / args.steps
     value = job_scenes / (ms_step * 1e-3)
+    if args.dump_outputs:
+        lat = pipe.latents_out(st).float().cpu().numpy()  # every rank: the view-sharded gather is collective
+        if rank == 0:
+            import numpy as np
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            np.save(os.path.join(args.dump_outputs, "latents.npy"), lat)
 
     # ---- end-to-end through the host-facing call.  A denoising step's inputs are (x_t, t): every timed step copies
     #      the scene's latents from pinned host memory to the device, runs the step (graph replay) and reads x_{t-1}
@@ -379,7 +390,7 @@ def main():
         ms_e2e, ms_full = tt[0].item(), tt[1].item()
     e2e_value = job_scenes / (ms_e2e / args.steps * 1e-3)
 
-    # ---- roofline of the dominant kernel (tcgen05 GEMM / implicit-GEMM conv): per-launch CUDA events, eager pass
+    # ---- roofline of the dominant kernel (wgmma GEMM / implicit-GEMM conv): per-launch CUDA events, eager pass
     pipe.use_cuda_graph = False
     overlap_was, pipe.overlap_controlnet = pipe.overlap_controlnet, False  # serial launches: per-kernel times are not inflated by co-running kernels
     st = prepare()
@@ -399,40 +410,32 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    # burst peak when the sampled clocks were un-capped (no power cap, SM clock at max): that is the regime the cuBLAS
-    # burst figure was taken in; the sustained figure otherwise
+    # measured peaks (MEASURED_PEAKS.json, if the machine provides one): the burst figure when the sampled clocks were
+    # un-capped (no power cap, SM clock at max), the sustained figure otherwise; else the H100 SXM data-sheet dense BF16 rate
     capped = ("sw_power_cap" in (clocks.get("reasons") or [])) or not clocks.get("sm_mhz") or \
         clocks["sm_mhz"] < 0.95 * (clocks.get("sm_max_mhz") or 1e9)
     if peaks:
         key = "bf16_tflops_sustained" if capped else "bf16_tflops"
-        peak_tf = peaks.get(key) or peaks.get("bf16_tflops_sustained") or 1400.0
+        peak_tf = peaks.get(key) or peaks.get("bf16_tflops_sustained") or 989.0
         peak_src = f"MEASURED_PEAKS.json {key} (of measured; clocks during the timed region {'capped' if capped else 'un-capped at max'})"
     else:
-        peak_tf = 1400.0 if capped else 1590.0
-        peak_src = "fallback " + ("1.4 PF/s sustained" if capped else "1.59 PF/s burst") + " (of fallback)"
+        peak_tf = 989.0
+        peak_src = "H100 SXM data sheet, dense BF16 at 700 W (not reached on a power-limited card)"
     g = [(f, s) for k, f, s in prof if k == "gemm_conv"]
     a = [(f, s) for k, f, s in prof if k == "attention"]
     gf, gs = sum(f for f, _ in g), sum(s for _, s in g)
     af, as_ = sum(f for f, _ in a), sum(s for _, s in a)
     achieved = gf / gs / 1e12 if gs > 0 else 0.0
-    traffic, traffic_src = None, None
-    try:  # per-launch DRAM bytes of the dominant kernel from this round's committed ncu capture, if one exists
-        tj = json.load(open(os.path.join(ROOT, "profiles", "traffic_r2.json")))
-        traffic, traffic_src = tj["dram_bytes_per_launch"], "profiles/traffic_r2.json (ncu dram__bytes_read+write per launch, committed capture)"
-    except Exception:
-        pass
     scale = args.scenes * views_local / 6
     alg_full = TFLOP_PER_SCENE_STEP_CFG[args.res] * scale
     d_core, d_kv = context_delta_tflop(args, 20)
     alg = alg_full if args.workload == "full" else alg_full - (d_core + d_kv) * views_local / 6
     _, kv_all = context_delta_tflop(args, 98 if args.workload == "full" else 78)
     hoisted = kv_all * views_local / 6
-    roofline = {"bound": "tensor", "kernel": "gemm_pair_kernel / gemm_tc2_kernel (tcgen05 GEMM / implicit-GEMM conv, all shapes of one step)",
+    roofline = {"bound": "tensor", "kernel": "gemm_wgmma_kernel (wgmma GEMM / implicit-GEMM conv, all shapes of one step)",
                 "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved / peak_tf, "peak_source": peak_src,
-                "launches": len(g), "flops_per_step": gf, "kernel_ms_per_step": gs * 1e3, "traffic": traffic,
-                "traffic_source": traffic_src,
-                "timing_note": "per-launch CUDA events on an eager pass queued behind a spin kernel (no host enqueue gaps); "
-                               "profiles/ has the ncu device times per shape",
+                "launches": len(g), "flops_per_step": gf, "kernel_ms_per_step": gs * 1e3,
+                "timing_note": "per-launch CUDA events on an eager pass queued behind a spin kernel (no host enqueue gaps)",
                 "attention": {"achieved": (af / as_ / 1e12 if as_ > 0 else 0.0), "launches": len(a),
                               "kernel_ms_per_step": as_ * 1e3, "flops_per_step": af},
                 "whole_step": {"algorithmic_tflop": alg, "hoisted_tflop": hoisted, "executed_tensor_tflop": (gf + af) / 1e12,
@@ -539,7 +542,7 @@ def main():
                                "dtype": "bf16", "speedup_of_value": value / (args.scenes / sec),
                                "note": "the unmodified reference pipeline (its own UNet2DConditionModelMultiview + BEVControlNetModel, "
                                        "oracle/_ref snapshot) on this GPU, CFG on, eager launches, attention = diffusers AttnProcessor2_0 "
-                                       "(torch SDPA; the vendored xformers has no sm_100 kernel), wall-clock between synchronised step callbacks"}
+                                       "(torch SDPA), wall-clock between synchronised step callbacks"}
         line = {"metric": metric, "value": value, "unit": "scene-steps/s", "n_gpus": n_gpus, "steps": args.steps,
                 "warmup": args.warmup, "ms_per_step": ms_step, "higher_is_better": True,
                 "scaling": "strong" if by_views else "weak", "vs_baseline": None, "dtype": "bf16",

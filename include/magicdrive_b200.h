@@ -1,5 +1,5 @@
 /*
- * magicdrive_b200 — C ABI of the B200-native multi-view denoising hot path.
+ * magicdrive_b200 — C ABI of the multi-view denoising hot path (CUDA kernels for sm_90a, NVIDIA H100).
  *
  * Every entry point takes raw device pointers, sizes, strides and a cudaStream_t (as void*), returns 0 on
  * success or a negative status, and never allocates, synchronises or takes ownership.  mdb_last_error()
@@ -9,7 +9,7 @@
  * The reference has no native boundary of its own for this path except one op: xformers'
  * efficient_attention_forward_cutlass (third_party/xformers/xformers/csrc/attention/attention.cpp:27,
  * attention_forward_generic.cu:330-334).  Everything else it runs is a torch.nn call; each function below
- * names the reference call site (file:line under /root/reference) it replaces.
+ * names the reference call site (file:line in the MagicDrive source tree) it replaces.
  */
 #ifndef MAGICDRIVE_B200_H
 #define MAGICDRIVE_B200_H
@@ -33,11 +33,11 @@ const char* mdb_last_error(void);
  * single-stream regions (the UNet up path); the environment variable MDB_PDL=0|1 overrides the flag. */
 int mdb_set_pdl(int on);
 int mdb_version(void);
-/* 1 if a CUDA device of compute capability 10.x is usable, else 0 (never raises). */
+/* 1 if a CUDA device of compute capability 9.0 (sm_90a) is usable, else 0 (never raises). */
 int mdb_device_ok(void);
 
 /* ------------------------------------------------------------------------------------------------
- * mdb_gemm_conv: tensor-core (tcgen05) GEMM / implicit-GEMM convolution with fused epilogue.
+ * mdb_gemm_conv: tensor-core (wgmma) GEMM / implicit-GEMM convolution with fused epilogue.
  *   out[pix, n] = scale * ( sum_{r,s,c} A[pix*stride + (r,s) - pad, c] * W[n, (r*taps_w+s)*C + c]
  *                           + bias[n] + rowbias[img(pix), n] ) + residual[pix, n]
  *   epi_mode 1 (GEGLU): W/bias are packed per 256-column tile as [128 value | 128 gate] and
@@ -72,10 +72,9 @@ typedef struct {
   size_t workspace_bytes;
   int force_block_n;    /* 0 = auto; test hook */
   int force_splits;     /* 0 = auto; test hook */
-  int kernel_variant;   /* 0 = auto (CTA-pair kernel where it applies, else the single-CTA split-K kernel); 2 = single-CTA
-                         * persistent kernel; 3 = CTA-pair kernel; 4 = the pair kernel's code on single CTAs; test / A-B hook */
-  int debug_flags;      /* ablation hook (0 in production): 1 skip stores, 2 skip epilogue loads, 4 skip TMEM loads */
-  void* trace;          /* debug: device int64[8*16] receiving per-CTA clock64 stamps of the persistent kernel, or NULL */
+  int kernel_variant;   /* 0 = auto (single CTAs, split-K where the planner wants it); 2 = the same; 3 = CTA pairs: 2-CTA
+                         * clusters on consecutive M tiles, each CTA TMA-loads half of the weight tile and multicasts it to
+                         * both (no split-K); 4 = single CTAs without split-K; test / A-B hook */
   /* LayerNorm folded into the GEMM (attention.py:85,104,120; blocks.py:67-71): A is the RAW tensor x, W was
    * pre-multiplied by gamma (W' = W * gamma), bias holds c_n = sum_k beta_k W[n,k] + b_n, and the epilogue applies
    *   out = rstd_row * (acc - mean_row * ln_colsum[n]) + c_n
@@ -139,11 +138,6 @@ int mdb_attention(const void* q, int ldq, const void* k, int ldk, const void* v,
 int mdb_attention_multi(const void* q, int ldq, int n_src, const void* const* k, const int* ldk, const void* const* v,
                         const int* ldv, const int* b_kv, void* out, int ldo, int b, int heads, int lq, int lk, int d,
                         const int* kv_index, int n_sets, float scale, void* stream);
-
-/* Debug hook (NULL in production): a device int64[3 * 16 * 8] buffer that receives clock64 stamps of the first CTA of
- * every following fused-attention launch (MMA warp and two softmax warps, 16 KV iterations, 8 points each);
- * tools/bench_attn.py --trace prints them.  Pass NULL to switch it off. */
-int mdb_attention_debug_trace(void* device_i64_384);
 
 /* out = a + b (bf16), n elements (unet_2d_condition_multiview.py:464-473, 487-488). */
 int mdb_add(const void* a, const void* b, void* out, long long n, void* stream);

@@ -28,7 +28,7 @@ class GemmDesc(C.Structure):
         ("out", C.c_void_p), ("ldo", C.c_int), ("out_is_f32", C.c_int), ("out_scale", C.c_float),
         ("epi_mode", C.c_int),
         ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
-        ("force_block_n", C.c_int), ("force_splits", C.c_int), ("kernel_variant", C.c_int), ("debug_flags", C.c_int), ("trace", C.c_void_p),
+        ("force_block_n", C.c_int), ("force_splits", C.c_int), ("kernel_variant", C.c_int),
         ("ln_stats", C.c_void_p), ("ln_parts", C.c_int), ("ln_eps", C.c_float), ("ln_colsum", C.c_void_p),
         ("stats_out", C.c_void_p),
     ]
@@ -49,7 +49,6 @@ SIGNATURES = {
     "mdb_layernorm": (_i, [_vp, _ll, _i, _i, _vp, _vp, _f, _vp, _i, _vp]),
     "mdb_attention": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _f, _vp]),
     "mdb_attention_multi": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _f, _vp]),
-    "mdb_attention_debug_trace": (_i, [_vp]),
     "mdb_add": (_i, [_vp, _vp, _vp, _ll, _vp]),
     "mdb_upsample_nearest": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp]),
     "mdb_adaptive_avgpool": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),

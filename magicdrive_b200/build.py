@@ -1,4 +1,4 @@
-"""Build the sm_100a C-ABI shared library in-tree with nvcc (no torch extension machinery).
+"""Build the sm_90a (H100) C-ABI shared library in-tree with nvcc (no torch extension machinery).
 
 `python -m magicdrive_b200.build` -> magicdrive_b200/lib/libmagicdrive_b200.so
 """
@@ -13,7 +13,7 @@ CSRC = ROOT / "csrc"
 LIBDIR = ROOT / "lib"
 LIB = LIBDIR / "libmagicdrive_b200.so"
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--use_fast_math",
 ]
 # --use_fast_math is NOT applied to the files listed here (exact erf/sin/cos/exp paths that parity tests pin)

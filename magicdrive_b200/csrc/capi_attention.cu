@@ -1,4 +1,4 @@
-// Fused multi-head attention forward (flash-style, online softmax in fp32) on tcgen05 + TMA: C-ABI launchers.
+// Fused multi-head attention forward (flash-style, online softmax in fp32) on wgmma + TMA: C-ABI launchers.
 //
 // Layout: q/out [B, Lq, heads*D] (row strides ldq/ldo), k/v [Bkv, Lk, heads*D] (ldk/ldv): exactly what the fused
 // QKV projection GEMM writes, so no head transpose is ever materialised.  With n_sets == 2 the kernel runs two
@@ -6,32 +6,28 @@
 // BasicMultiviewTransformerBlock (magicdrive/networks/blocks.py:112-121, 213-217).  K/V may be spread over up to three
 // buffers (mdb_attention_multi): in view-sharded runs the neighbour views' K/V are read in place from the ring-neighbour
 // GPUs' buffers through NVLink peer memory (the tensor maps simply point at peer-mapped addresses).
-// Kernels: attention_tc2.cuh (head dim <= 80, production), attention_tc.cuh (head dim 160, and the A/B variant "tc").
+// Kernel: attention_wgmma.cuh.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
 #include <stdlib.h>
+#include <string.h>
 
 #include "../../include/magicdrive_b200.h"
 #define MDB_NEED_TENSORMAP
 #include "common_host.h"
-#include <string.h>
-#include "attention_tc.cuh"
-#include "attention_tc2.cuh"
-
-static long long* g_attn_trace = nullptr;  // debug: device int64[3*16*8] for attention_tc2's phase stamps (mdb_attention_debug_trace)
+#include "attention_wgmma.cuh"
 
 namespace {
 
-// ---------------------------------------------------------------- tcgen05 path
-// [B, L, heads*D] (row stride ld) as a 4-D map (d, head, token, batch); box = (64, 1, 128, 1): the head dim is
+// [B, L, heads*D] (row stride ld) as a 4-D map (d, head, token, batch); box = (64, 1, rows, 1): the head dim is
 // zero-padded to 64-wide chunks by TMA out-of-bounds fill, rows beyond L are zero-filled too.
-bool make_qkv_map(CUtensorMap* m, const void* ptr, int d, int heads, int l, int b, int ld) {
+bool make_qkv_map(CUtensorMap* m, const void* ptr, int d, int heads, int l, int b, int ld, int rows) {
   mdb::EncodeTiledFn enc = mdb::get_encode();
   if (!enc) return false;
   cuuint64_t dims[4] = {(cuuint64_t)d, (cuuint64_t)heads, (cuuint64_t)l, (cuuint64_t)b};
   cuuint64_t strides[3] = {(cuuint64_t)d * 2, (cuuint64_t)ld * 2, (cuuint64_t)l * ld * 2};
-  cuuint32_t box[4] = {64u, 1u, (cuuint32_t)mdb::ATT_BM, 1u};
+  cuuint32_t box[4] = {64u, 1u, (cuuint32_t)rows, 1u};
   cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
   return enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr,
              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -45,11 +41,11 @@ struct KvSources {
   int n;
 };
 
-bool make_kv_maps(mdb::AttnKvMaps* m, const KvSources& s, int d, int heads, int lk) {
+bool make_kv_maps(mdb::AttnKvMaps* m, const KvSources& s, int d, int heads, int lk, int rows) {
   for (int i = 0; i < mdb::ATT_MAX_SRC; ++i) {
     const int j = i < s.n ? i : 0;  // unused slots alias source 0
-    if (!make_qkv_map(&m->k[i], s.k[j], d, heads, lk, s.b_kv[j], s.ldk[j]) ||
-        !make_qkv_map(&m->v[i], s.v[j], d, heads, lk, s.b_kv[j], s.ldv[j]))
+    if (!make_qkv_map(&m->k[i], s.k[j], d, heads, lk, s.b_kv[j], s.ldk[j], rows) ||
+        !make_qkv_map(&m->v[i], s.v[j], d, heads, lk, s.b_kv[j], s.ldv[j], rows))
       return false;
   }
   return true;
@@ -60,20 +56,20 @@ int attn_num_sms() {
   if (!sms) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
   }
   return sms;
 }
 
-// Query tiles per CTA walk (AttnTcParams::q_step) for the single-S tc2 kernel when one K/V tile covers all keys: as many
-// CTAs as two per SM, each keeping its K/V tile and walking ~nq / gx query tiles.  0 = one tile per CTA.  MDB_ATTN_MULTIQ=0 disables (A/B).
-int multi_q_step(int b, int heads, int lq, int lk, int n_sets) {
-  if (lk > mdb::ATT_BN || n_sets != 1) return 0;
+// Query tiles per CTA walk (AttnParams::q_step) when one K/V tile covers all keys: one CTA per SM, each keeping its K/V tile
+// and walking ~nq / gx query tiles.  0 = one tile per CTA.  MDB_ATTN_MULTIQ=0 disables it.
+int multi_q_step(int b, int heads, int lq, int lk, int n_sets, int bn) {
+  if (lk > bn || n_sets != 1) return 0;
   const char* e = getenv("MDB_ATTN_MULTIQ");
   if (e && e[0] == '0') return 0;
   const int nq = (lq + mdb::ATT_BM - 1) / mdb::ATT_BM;
   const long long per_tile_ctas = static_cast<long long>(b) * heads;
-  const long long slots = 2LL * attn_num_sms();
+  const long long slots = attn_num_sms();
   if (per_tile_ctas * nq <= slots) return 0;  // everything is co-resident anyway
   long long gx = slots / per_tile_ctas;
   if (gx < 1) gx = 1;
@@ -81,88 +77,56 @@ int multi_q_step(int b, int heads, int lq, int lk, int n_sets) {
   return static_cast<int>(gx);
 }
 
-template <typename Cfg, typename Kernel>
-int launch_tc(Kernel kernel, const char* name, const void* q, int ldq, const KvSources& src, void* out, int ldo, int b, int heads,
-              int lq, int lk, int d, const int* kv_index, int n_sets, float scale, cudaStream_t st, bool* attr, bool allow_multi_q = false) {
-  if (!*attr) {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
-    if (e != cudaSuccess) return mdb::set_error(MDB_ERR_CUDA, "%s smem attr: %s", name, cudaGetErrorString(e));
-    *attr = true;
+template <int D, int BN_>
+int launch_attention(const void* q, int ldq, const KvSources& src, void* out, int ldo, int b, int heads, int lq, int lk,
+                     const int* kv_index, int n_sets, float scale, cudaStream_t st) {
+  using Cfg = mdb::AttnCfg<D, BN_>;
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t e = cudaFuncSetAttribute(mdb::attention_wgmma_kernel<D, BN_>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+    if (e != cudaSuccess) return mdb::set_error(MDB_ERR_CUDA, "attention_wgmma_kernel smem attr: %s", cudaGetErrorString(e));
+    attr = true;
   }
   CUtensorMap tq;
   mdb::AttnKvMaps kvm;
-  if (!make_qkv_map(&tq, q, d, heads, lq, b, ldq) || !make_kv_maps(&kvm, src, d, heads, lk))
-    return mdb::set_error(MDB_ERR_CUDA, "mdb_attention: cuTensorMapEncodeTiled failed (d=%d heads=%d lq=%d lk=%d)", d, heads, lq, lk);
-  mdb::AttnTcParams p;
+  if (!make_qkv_map(&tq, q, D, heads, lq, b, ldq, mdb::ATT_BM) || !make_kv_maps(&kvm, src, D, heads, lk, Cfg::BN))
+    return mdb::set_error(MDB_ERR_CUDA, "mdb_attention: cuTensorMapEncodeTiled failed (d=%d heads=%d lq=%d lk=%d)", D, heads, lq, lk);
+  mdb::AttnParams p;
   p.out = static_cast<__nv_bfloat16*>(out);
   p.ldo = ldo, p.lq = lq, p.lk = lk, p.kv_index = kv_index, p.n_sets = n_sets, p.n_src = src.n;
   p.scale_log2 = scale * 1.4426950408889634f;
-  p.trace = g_attn_trace;
-  p.q_step = allow_multi_q ? multi_q_step(b, heads, lq, lk, n_sets) : 0;
+  p.q_step = multi_q_step(b, heads, lq, lk, n_sets, Cfg::BN);
   dim3 grid(p.q_step > 0 ? p.q_step : (lq + mdb::ATT_BM - 1) / mdb::ATT_BM, heads, b);
-  cudaError_t le = mdb::launch_pdl(kernel, grid, dim3(Cfg::kThreads), Cfg::kSmemBytes, st, tq, kvm, p);
-  if (le != cudaSuccess) return mdb::set_error(MDB_ERR_CUDA, "%s launch: %s", name, cudaGetErrorString(le));
+  cudaError_t le = mdb::launch_pdl(mdb::attention_wgmma_kernel<D, BN_>, grid, dim3(Cfg::kThreads), Cfg::kSmemBytes, st, tq, kvm, p);
+  if (le != cudaSuccess) return mdb::set_error(MDB_ERR_CUDA, "attention_wgmma_kernel launch: %s", cudaGetErrorString(le));
   cudaError_t e2 = cudaGetLastError();
-  if (e2 != cudaSuccess) return mdb::set_error(MDB_ERR_CUDA, "%s: %s", name, cudaGetErrorString(e2));
+  if (e2 != cudaSuccess) return mdb::set_error(MDB_ERR_CUDA, "attention_wgmma_kernel: %s", cudaGetErrorString(e2));
   return MDB_OK;
 }
 
-template <int D>
-int launch_attention_tc(const void* q, int ldq, const KvSources& src, void* out, int ldo, int b, int heads, int lq, int lk,
-                        const int* kv_index, int n_sets, float scale, cudaStream_t st) {
-  static bool attr = false;
-  return launch_tc<mdb::AttnTcCfg<D>>(mdb::attention_tc_kernel<D>, "attention_tc_kernel", q, ldq, src, out, ldo, b, heads, lq, lk, D,
-                                      kv_index, n_sets, scale, st, &attr);
-}
-
-template <int D, bool DOUBLE_S>
-int launch_attention_tc2(const void* q, int ldq, const KvSources& src, void* out, int ldo, int b, int heads, int lq, int lk,
-                         const int* kv_index, int n_sets, float scale, cudaStream_t st) {
-  if constexpr (!DOUBLE_S) {
-    if (multi_q_step(b, heads, lq, lk, n_sets) > 0) {  // one K/V tile, more query tiles than CTA slots: multi-Q instantiation
-      static bool attr_mq = false;
-      return launch_tc<mdb::AttnTc2Cfg<D, false>>(mdb::attention_tc2_kernel<D, false, true>, "attention_tc2_kernel<multi-Q>", q, ldq, src,
-                                                  out, ldo, b, heads, lq, lk, D, kv_index, n_sets, scale, st, &attr_mq, true);
-    }
+template <int BN_>
+int attention_dispatch_bn(const void* q, int ldq, const KvSources& src, void* out, int ldo, int b, int heads, int lq, int lk, int d,
+                          const int* kv_index, int n_sets, float scale, cudaStream_t st) {
+  switch (d) {
+    case 32: return launch_attention<32, BN_>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
+    case 40: return launch_attention<40, BN_>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
+    case 64: return launch_attention<64, BN_>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
+    case 80: return launch_attention<80, BN_>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
+    case 160: return launch_attention<160, BN_>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
+    default: return mdb::set_error(MDB_ERR_UNSUPPORTED, "mdb_attention: head dim %d not instantiated (32, 40, 64, 80, 160)", d);
   }
-  static bool attr = false;
-  return launch_tc<mdb::AttnTc2Cfg<D, DOUBLE_S>>(mdb::attention_tc2_kernel<D, DOUBLE_S, false>, "attention_tc2_kernel", q, ldq, src, out,
-                                                 ldo, b, heads, lq, lk, D, kv_index, n_sets, scale, st, &attr, false);
 }
 
-// Which kernel generation serves a call: MDB_ATTN_KERNEL = tc2 | tc2d | tc (A/B switch, read per call).
-enum class AttnKernel { kTc, kTc2, kTc2Double };
-AttnKernel attention_kernel_choice() {
-  const char* e = getenv("MDB_ATTN_KERNEL");
-  if (e && !strcmp(e, "tc2d")) return AttnKernel::kTc2Double;
-  if (e && !strcmp(e, "tc")) return AttnKernel::kTc;
-  return AttnKernel::kTc2;  // default: tc2 (two CTAs/SM, one S buffer) for d <= 64, double-buffered S for d = 80, tc for d = 160
-}
-
+// Key-tile width (A/B switch, read per call): MDB_ATTN_KERNEL = tc2 (default: 128 keys for head dims <= 64, 64 above) |
+// tc2d (64-key tiles: smaller S fragment, deeper K/V ring) | tc (128-key tiles for every head dim).
 int attention_dispatch(const void* q, int ldq, const KvSources& src, void* out, int ldo, int b, int heads, int lq, int lk, int d,
                        const int* kv_index, int n_sets, float scale, cudaStream_t st) {
-  using namespace mdb;
-  const AttnKernel which = attention_kernel_choice();
-#define MDB_TC2(DD, DBL) return launch_attention_tc2<DD, DBL>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st)
-  if (which != AttnKernel::kTc) {
-    const bool dbl = which == AttnKernel::kTc2Double;  // tc2: two CTAs/SM with one S buffer where d <= 64
-    switch (d) {
-      case 40: if (dbl) MDB_TC2(40, true); else MDB_TC2(40, false);
-      case 32: if (dbl) MDB_TC2(32, true); else MDB_TC2(32, false);
-      case 64: if (dbl) MDB_TC2(64, true); else MDB_TC2(64, false);
-      case 80: MDB_TC2(80, true);
-      default: break;  // d = 160 stays on the first tcgen05 kernel
-    }
-  }
-#undef MDB_TC2
-  switch (d) {
-    case 40: return launch_attention_tc<40>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
-    case 80: return launch_attention_tc<80>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
-    case 160: return launch_attention_tc<160>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
-    case 32: return launch_attention_tc<32>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
-    case 64: return launch_attention_tc<64>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
-    default: return set_error(MDB_ERR_UNSUPPORTED, "mdb_attention: head dim %d not instantiated (32, 40, 64, 80, 160)", d);
-  }
+  const char* e = getenv("MDB_ATTN_KERNEL");
+  if (e && !strcmp(e, "tc2d")) return attention_dispatch_bn<64>(q, ldq, src, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, scale, st);
+  if (e && !strcmp(e, "tc")) return attention_dispatch_bn<128>(q, ldq, src, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, scale, st);
+  if (e && *e && strcmp(e, "tc2"))
+    return mdb::set_error(MDB_ERR_INVALID, "mdb_attention: MDB_ATTN_KERNEL must be tc2, tc2d or tc (got %s)", e);
+  return attention_dispatch_bn<0>(q, ldq, src, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, scale, st);
 }
 
 }  // namespace
@@ -193,9 +157,4 @@ extern "C" int mdb_attention(const void* q, int ldq, const void* k, int ldk, con
                              int b_kv, int heads, int lq, int lk, int d, const int* kv_index, int n_sets, float scale,
                              void* stream) {
   return mdb_attention_multi(q, ldq, 1, &k, &ldk, &v, &ldv, &b_kv, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, scale, stream);
-}
-
-extern "C" int mdb_attention_debug_trace(void* device_i64_384) {
-  g_attn_trace = static_cast<long long*>(device_i64_384);
-  return MDB_OK;
 }

@@ -1,4 +1,4 @@
-// C-ABI launcher for the tcgen05 GEMM / implicit-GEMM convolution (include/magicdrive_b200.h: mdb_gemm_conv).
+// C-ABI launcher for the wgmma GEMM / implicit-GEMM convolution (include/magicdrive_b200.h: mdb_gemm_conv).
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdio.h>
@@ -10,8 +10,7 @@
 #include "../../include/magicdrive_b200.h"
 #define MDB_NEED_TENSORMAP
 #include "common_host.h"
-#include "gemm_tc2.cuh"
-#include "gemm_pair.cuh"
+#include "gemm_wgmma.cuh"
 
 using namespace mdb;
 
@@ -47,6 +46,7 @@ bool make_w_map(CUtensorMap* m, const void* ptr, int n_out, int k, int block_n) 
 
 struct Plan {
   int bn, bh, bw, tiles_n, tiles_h, tiles_w;
+  int ctas, m_groups;  // CTAs per cluster (1, or 2 = CTA pairs) and M-tile groups walked by one cluster
   int block_n, n_tiles, splits, kb_per_split, kb_total;
 };
 
@@ -55,7 +55,7 @@ int num_sms() {
   if (!sms) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
   }
   return sms;
 }
@@ -96,6 +96,8 @@ int validate(const mdb_gemm_desc* d) {
     return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: leading dimensions must be multiples of 8");
   if (d->n_out % 8) return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: n_out must be a multiple of 8");
   if (d->stride != 1 && d->stride != 2) return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: stride must be 1 or 2");
+  if (d->kernel_variant != 0 && (d->kernel_variant < 2 || d->kernel_variant > 4))
+    return set_error(MDB_ERR_INVALID, "mdb_gemm_conv: kernel_variant must be 0, 2, 3 or 4");
   if (d->n_img <= 0 || d->h_out <= 0 || d->w_out <= 0 || d->taps_h <= 0 || d->taps_w <= 0)
     return set_error(MDB_ERR_INVALID, "mdb_gemm_conv: bad shape");
   if ((reinterpret_cast<uintptr_t>(d->a0) | reinterpret_cast<uintptr_t>(d->a1) | reinterpret_cast<uintptr_t>(d->w) |
@@ -107,11 +109,15 @@ int validate(const mdb_gemm_desc* d) {
   return MDB_OK;
 }
 
-void make_plan(const mdb_gemm_desc* d, Plan* pl) {
+// Tile width / split-K plan for `ctas` CTAs per cluster.
+void plan_for(const mdb_gemm_desc* d, int ctas, bool allow_split, Plan* pl) {
   choose_box(d->n_img, d->h_out, d->w_out, pl);
   const int m_tiles = pl->tiles_n * pl->tiles_h * pl->tiles_w;
+  pl->ctas = ctas;
+  pl->m_groups = (m_tiles + ctas - 1) / ctas;
   pl->kb_total = d->taps_h * d->taps_w * ((d->c0 + d->c1) / 64);
   const int sms = num_sms();
+  const int clusters = sms / ctas;
   int bn_choice = 0;
   if (d->epi_mode == 1) {
     bn_choice = 256;
@@ -122,11 +128,11 @@ void make_plan(const mdb_gemm_desc* d, Plan* pl) {
     double best = 1e30;
     for (int i = 0; i < 4; ++i) {
       const int bn = cands[i];
-      if (bn == 64 && d->n_out >= 128) continue;  // 64-wide tiles re-read A too often (measured: 4x7 convs 56 -> 40 us)
+      if (bn == 64 && d->n_out >= 128) continue;  // 64-wide tiles re-read A too often
       const int nt = (d->n_out + bn - 1) / bn;
-      const long long ctas = (long long)m_tiles * nt;
-      const long long waves = (ctas + sms - 1) / sms;
-      // cost ~ waves * (MMA time ~ bn, floored by the A-side smem/issue cost) ; prefer big tiles on ties
+      const long long groups = (long long)pl->m_groups * nt;
+      const long long waves = (groups + clusters - 1) / clusters;
+      // cost ~ waves * (MMA time ~ bn, floored by the A-side cost) ; prefer big tiles on ties
       const double cost = (double)waves * (bn < 96 ? 96 : bn) * 1.0 + (double)waves * 6.0;
       if (cost < best - 1e-9) best = cost, bn_choice = bn;
     }
@@ -135,11 +141,13 @@ void make_plan(const mdb_gemm_desc* d, Plan* pl) {
   pl->n_tiles = (d->n_out + bn_choice - 1) / bn_choice;
   // split-K when the grid cannot fill the machine and K is deep
   int splits = 1;
-  const long long ctas = (long long)m_tiles * pl->n_tiles;
-  if (d->force_splits > 0) {
+  const long long ctas_total = (long long)m_tiles * pl->n_tiles;
+  if (!allow_split) {
+    splits = 1;
+  } else if (d->force_splits > 0) {
     splits = d->force_splits;
-  } else if (d->epi_mode == 0 && d->workspace && ctas * 2 <= sms && pl->kb_total >= 16) {
-    splits = (int)(sms / ctas);
+  } else if (d->epi_mode == 0 && !d->ln_stats && !d->stats_out && d->workspace && ctas_total * 2 <= sms && pl->kb_total >= 16) {
+    splits = (int)(sms / ctas_total);
     if (splits > pl->kb_total / 8) splits = pl->kb_total / 8;
     if (splits > 16) splits = 16;
     if (splits < 1) splits = 1;
@@ -147,117 +155,30 @@ void make_plan(const mdb_gemm_desc* d, Plan* pl) {
   if (splits > pl->kb_total) splits = pl->kb_total;
   if (splits > 1) {
     const size_t need = (size_t)splits * d->n_img * d->h_out * d->w_out * d->n_out * sizeof(float);
-    if (!d->workspace || d->workspace_bytes < need || d->epi_mode != 0) splits = 1;
+    if (!d->workspace || d->workspace_bytes < need || d->epi_mode != 0 || d->ln_stats || d->stats_out) splits = 1;
   }
   pl->kb_per_split = (pl->kb_total + splits - 1) / splits;
   pl->splits = (pl->kb_total + pl->kb_per_split - 1) / pl->kb_per_split;  // no empty split
 }
 
-template <int BN>
-int launch2(const Plan& pl, const CUtensorMap& tA0, const CUtensorMap& tA1, const CUtensorMap& tB, const GemmParams& gp,
-            cudaStream_t st) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tc2_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         GemmCfg2<BN>::kSmemBytes);
-    if (e != cudaSuccess) return set_error(MDB_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-    attr_set = true;
-  }
-  GemmParams2 pp;
-  pp.p = gp;
-  pp.m_tiles = pl.tiles_n * pl.tiles_h * pl.tiles_w;
-  pp.n_tiles = pl.n_tiles;
-  pp.splits = pl.splits;
-  const long long total = (long long)pp.m_tiles * pp.n_tiles * pp.splits;
-  const int sms = num_sms();
-  const int grid = (int)(total < sms ? total : sms);
-  cudaError_t e = launch_pdl(gemm_tc2_kernel<BN>, dim3(grid), dim3(GemmCfg2<BN>::kThreads), GemmCfg2<BN>::kSmemBytes, st, tA0,
-                             tA1, tB, pp);
-  if (e == cudaSuccess) e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error(MDB_ERR_CUDA, "gemm_tc2_kernel<%d> launch: %s", BN, cudaGetErrorString(e));
-  return MDB_OK;
-}
-
-
-// 4-D map over a [n_img, h, w, ld] bf16 tensor using the first `cols` channels, 32-column boxes with the 64-byte swizzle:
-// the staging boxes of gemm_pair_kernel's epilogue (TMA store of the output, TMA load of the residual).
-bool make_io_map(CUtensorMap* m, const void* ptr, int cols, int ld, int n, int h, int w, int bn, int bh, int bw) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return false;
-  cuuint64_t dims[4] = {(cuuint64_t)cols, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
-  cuuint64_t strides[3] = {(cuuint64_t)ld * 2, (cuuint64_t)w * ld * 2, (cuuint64_t)h * w * ld * 2};
-  cuuint32_t box[4] = {32u, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bn};
-  cuuint32_t estr[4] = {1u, 1u, 1u, 1u};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS;
-}
-
-struct Plan3 {
-  int bn, bh, bw, tiles_n, tiles_h, tiles_w;
-  int ctas, block_n, n_tiles, m_tiles, m_groups;
-};
-
-// Can gemm_pair_kernel run this descriptor at all (bf16 output through 32-column TMA boxes, one image per tile when a
-// per-image shift is used)?
-bool pair_supported(const mdb_gemm_desc* d, const Plan& box) {
-  if (d->out_is_f32 || d->epi_mode > 1) return false;
-  const int out_cols = d->epi_mode == 1 ? d->n_out / 2 : d->n_out;
-  if (out_cols % 32 || d->n_out % 32) return false;
-  if (d->rowbias && d->rowbias_ld != 0 && box.bn != 1) return false;
-  // bias / per-image shift / folded-LayerNorm column sums reach the epilogue as bulk copies of whole tiles: 16-byte alignment
-  auto misaligned = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15u) != 0; };
-  if (misaligned(d->bias) || misaligned(d->rowbias) || misaligned(d->ln_colsum) || (d->rowbias && d->rowbias_ld % 4)) return false;
-  return true;
-}
-
-// ceil(2^32 / d): x / d == umulhi(x, magic) whenever x * d < 2^32
-inline uint32_t div_magic(int d) { return static_cast<uint32_t>((0x100000000ULL + static_cast<uint32_t>(d) - 1) / static_cast<uint32_t>(d)); }
-
-void make_plan3(const mdb_gemm_desc* d, int ctas, Plan3* pl) {
-  Plan box;
-  choose_box(d->n_img, d->h_out, d->w_out, &box);
-  pl->bn = box.bn, pl->bh = box.bh, pl->bw = box.bw;
-  pl->tiles_n = box.tiles_n, pl->tiles_h = box.tiles_h, pl->tiles_w = box.tiles_w;
-  pl->ctas = ctas;
-  pl->m_tiles = box.tiles_n * box.tiles_h * box.tiles_w;
-  pl->m_groups = (pl->m_tiles + ctas - 1) / ctas;
-  const int clusters = num_sms() / ctas;
-  int bn_choice = 0;
-  if (d->epi_mode == 1) {
-    bn_choice = 256;
-  } else if (d->force_block_n) {
-    bn_choice = d->force_block_n;
-  } else {
-    const int cands[4] = {256, 160, 128, 64};
-    double best = 1e30;
-    for (int i = 0; i < 4; ++i) {
-      const int bn = cands[i];
-      if (bn == 64 && d->n_out >= 128) continue;
-      const int nt = (d->n_out + bn - 1) / bn;
-      const long long groups = (long long)pl->m_groups * nt;
-      const long long waves = (groups + clusters - 1) / clusters;
-      // tile time ~ BLOCK_N (MMA) with a floor for the A-side cost, plus a per-tile constant; big tiles win ties
-      const double cost = (double)waves * ((bn < 96 ? 96 : bn) + 8.0);
-      if (cost < best - 1e-9) best = cost, bn_choice = bn;
-    }
-  }
-  pl->block_n = bn_choice;
-  pl->n_tiles = (d->n_out + bn_choice - 1) / bn_choice;
+// kernel_variant: 0 / 2 = single CTAs (split-K allowed), 3 = CTA pairs, 4 = single CTAs without split-K.  Single CTAs are the
+// default because they measured faster on H100: the whole denoising step takes 18.4 ms with them and 25.6 ms with CTA pairs
+// (bench.py, H100 SXM).
+void make_plan(const mdb_gemm_desc* d, Plan* pl) {
+  if (d->kernel_variant == 3) return plan_for(d, 2, false, pl);
+  plan_for(d, 1, d->kernel_variant != 4, pl);
 }
 
 template <int BN, int CTAS>
-int launch3(const Plan3& pl, const CUtensorMap& tA0, const CUtensorMap& tA1, const CUtensorMap& tB, const CUtensorMap& tO,
-            const CUtensorMap& tR, const GemmParams3& gp, cudaStream_t st) {
-  using Cfg = PairCfg<BN, CTAS>;
+int launch(const CUtensorMap& tA0, const CUtensorMap& tA1, const CUtensorMap& tB, const GemmParams& gp, cudaStream_t st) {
+  using Cfg = WgGemmCfg<BN, CTAS>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_pair_kernel<BN, CTAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
-    if (e != cudaSuccess) return set_error(MDB_ERR_CUDA, "cudaFuncSetAttribute(gemm_pair): %s", cudaGetErrorString(e));
+    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, CTAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+    if (e != cudaSuccess) return set_error(MDB_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     attr_set = true;
   }
-  const long long total = (long long)pl.m_groups * pl.n_tiles;
+  const long long total = (long long)gp.m_groups * gp.n_tiles * gp.splits;  // tiles per cluster walk
   const int clusters_max = num_sms() / CTAS;
   const int clusters = (int)(total < clusters_max ? total : clusters_max);
   cudaLaunchConfig_t cfg = {};
@@ -271,34 +192,22 @@ int launch3(const Plan3& pl, const CUtensorMap& tA0, const CUtensorMap& tA1, con
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   add_pdl_attr(cfg, attr, 1);
-  cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_pair_kernel<BN, CTAS>, tA0, tA1, tB, tO, tR, gp);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<BN, CTAS>, tA0, tA1, tB, gp);
   if (e == cudaSuccess) e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error(MDB_ERR_CUDA, "gemm_pair_kernel<%d,%d> launch: %s", BN, CTAS, cudaGetErrorString(e));
+  if (e != cudaSuccess) return set_error(MDB_ERR_CUDA, "gemm_wgmma_kernel<%d,%d> launch: %s", BN, CTAS, cudaGetErrorString(e));
   return MDB_OK;
 }
 
 template <int CTAS>
-int launch3_bn(const Plan3& pl, const CUtensorMap& tA0, const CUtensorMap& tA1, const CUtensorMap& tB, const CUtensorMap& tO,
-               const CUtensorMap& tR, const GemmParams3& gp, cudaStream_t st) {
-  switch (pl.block_n) {
-    case 256: return launch3<256, CTAS>(pl, tA0, tA1, tB, tO, tR, gp, st);
-    case 160: return launch3<160, CTAS>(pl, tA0, tA1, tB, tO, tR, gp, st);
-    case 128: return launch3<128, CTAS>(pl, tA0, tA1, tB, tO, tR, gp, st);
-    case 64: return launch3<64, CTAS>(pl, tA0, tA1, tB, tO, tR, gp, st);
-    default: return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: unsupported block_n %d", pl.block_n);
+int launch_bn(int block_n, const CUtensorMap& tA0, const CUtensorMap& tA1, const CUtensorMap& tB, const GemmParams& gp,
+              cudaStream_t st) {
+  switch (block_n) {
+    case 256: return launch<256, CTAS>(tA0, tA1, tB, gp, st);
+    case 160: return launch<160, CTAS>(tA0, tA1, tB, gp, st);
+    case 128: return launch<128, CTAS>(tA0, tA1, tB, gp, st);
+    case 64: return launch<64, CTAS>(tA0, tA1, tB, gp, st);
+    default: return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: unsupported block_n %d", block_n);
   }
-}
-
-// 0 = gemm_tc2 (split-K capable, fp32 / narrow outputs), 1 / 2 = gemm_pair with that many CTAs per tile group
-int choose_kernel(const mdb_gemm_desc* d, const Plan& old_plan) {
-  const bool wants_fold = d->ln_stats != nullptr || d->stats_out != nullptr;
-  if (!pair_supported(d, old_plan)) return 0;
-  if (wants_fold) return d->kernel_variant == 4 ? 1 : 2;  // only gemm_pair_kernel has the folded-LayerNorm epilogue
-  if (d->kernel_variant == 2) return 0;
-  if (d->kernel_variant == 3) return 2;
-  if (d->kernel_variant == 4) return 1;
-  if (old_plan.splits > 1) return 0;  // few tiles and a deep K: split-K on the single-CTA kernel fills the machine
-  return 2;
 }
 
 }  // namespace
@@ -307,7 +216,6 @@ extern "C" int mdb_gemm_conv_launches(const mdb_gemm_desc* d) {
   if (validate(d) != MDB_OK) return MDB_ERR_INVALID;
   Plan pl;
   make_plan(d, &pl);
-  if (choose_kernel(d, pl) != 0) return 1;
   return pl.splits > 1 ? 2 : 1;
 }
 
@@ -315,77 +223,18 @@ extern "C" int mdb_gemm_conv_stats_parts(const mdb_gemm_desc* d) {
   if (validate(d) != MDB_OK) return MDB_ERR_INVALID;
   Plan pl;
   make_plan(d, &pl);
-  const int k = choose_kernel(d, pl);
-  if (k == 0) return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv_stats_parts: this descriptor runs on the split-K kernel, which emits no row statistics");
-  Plan3 p3;
-  make_plan3(d, k, &p3);
-  return MDB_EPI_GROUPS * p3.n_tiles;
+  return pl.n_tiles;  // one (sum, sum sq) slot per row and N tile
 }
 
 extern "C" int mdb_gemm_conv(const mdb_gemm_desc* d, void* stream) {
   int rc = validate(d);
   if (rc != MDB_OK) return rc;
+  if (d->ln_stats && (d->taps_h != 1 || d->taps_w != 1 || !d->ln_colsum || d->ln_parts <= 0))
+    return set_error(MDB_ERR_INVALID, "mdb_gemm_conv: a folded LayerNorm needs a 1x1 GEMM, ln_colsum and ln_parts");
   Plan pl;
   make_plan(d, &pl);
+  if (d->epi_mode == 1 && pl.block_n != 256) return set_error(MDB_ERR_UNSUPPORTED, "GEGLU needs block_n 256");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int kernel = choose_kernel(d, pl);
-  if (kernel == 0 && (d->ln_stats || d->stats_out))
-    return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: folded LayerNorm / row statistics need the bf16 32-column-box kernel "
-                                          "(n_out %% 32 == 0, bf16 output)");
-  if (kernel != 0) {
-    Plan3 p3;
-    make_plan3(d, kernel, &p3);
-    if (d->epi_mode == 1 && p3.block_n != 256) return set_error(MDB_ERR_UNSUPPORTED, "GEGLU needs block_n 256");
-    if (d->ln_stats && (d->taps_h != 1 || d->taps_w != 1 || !d->ln_colsum || d->ln_parts <= 0))
-      return set_error(MDB_ERR_INVALID, "mdb_gemm_conv: a folded LayerNorm needs a 1x1 GEMM, ln_colsum and ln_parts");
-    CUtensorMap tA0, tA1, tB, tO, tR;
-    if (!make_act_map(&tA0, d->a0, d->c0, d->lda0, d->n_img, d->h_in, d->w_in, p3.bn, p3.bh, p3.bw, d->stride))
-      return set_error(MDB_ERR_CUDA, "cuTensorMapEncodeTiled(A0) failed (c=%d ld=%d n=%d h=%d w=%d box=%dx%dx%d s=%d)", d->c0,
-                       d->lda0, d->n_img, d->h_in, d->w_in, p3.bn, p3.bh, p3.bw, d->stride);
-    if (d->c1 > 0) {
-      if (!make_act_map(&tA1, d->a1, d->c1, d->lda1, d->n_img, d->h_in, d->w_in, p3.bn, p3.bh, p3.bw, d->stride))
-        return set_error(MDB_ERR_CUDA, "cuTensorMapEncodeTiled(A1) failed");
-    } else {
-      tA1 = tA0;
-    }
-    const int ktot3 = d->taps_h * d->taps_w * (d->c0 + d->c1);
-    if (!make_w_map(&tB, d->w, d->n_out, ktot3, p3.block_n / p3.ctas))
-      return set_error(MDB_ERR_CUDA, "cuTensorMapEncodeTiled(W) failed (n=%d k=%d)", d->n_out, ktot3);
-    const int out_cols = d->epi_mode == 1 ? d->n_out / 2 : d->n_out;
-    if (!make_io_map(&tO, d->out, out_cols, d->ldo, d->n_img, d->h_out, d->w_out, p3.bn, p3.bh, p3.bw))
-      return set_error(MDB_ERR_CUDA, "cuTensorMapEncodeTiled(out) failed (cols=%d ld=%d)", out_cols, d->ldo);
-    if (d->residual) {
-      if (!make_io_map(&tR, d->residual, d->n_out, d->ldr, d->n_img, d->h_out, d->w_out, p3.bn, p3.bh, p3.bw))
-        return set_error(MDB_ERR_CUDA, "cuTensorMapEncodeTiled(residual) failed (ld=%d)", d->ldr);
-    } else {
-      tR = tO;
-    }
-    GemmParams3 g3;
-    memset(&g3, 0, sizeof(g3));
-    GemmParams& gp = g3.p;
-    gp.n_img = d->n_img, gp.h_out = d->h_out, gp.w_out = d->w_out, gp.n_out = d->n_out;
-    gp.taps_h = d->taps_h, gp.taps_w = d->taps_w, gp.stride = d->stride, gp.pad_h = d->pad_h, gp.pad_w = d->pad_w;
-    gp.cblocks0 = d->c0 / 64, gp.cblocks1 = d->c1 / 64;
-    gp.bn = p3.bn, gp.bh = p3.bh, gp.bw = p3.bw, gp.tiles_h = p3.tiles_h, gp.tiles_w = p3.tiles_w;
-    gp.epi_mode = d->epi_mode;
-    gp.bias = d->bias, gp.rowbias = d->rowbias, gp.rowbias_ld = d->rowbias_ld;
-    gp.out = d->out, gp.ldo = d->ldo, gp.out_scale = d->out_scale;
-    gp.trace = static_cast<long long*>(d->trace);
-    g3.m_tiles = p3.m_tiles, g3.m_groups = p3.m_groups, g3.n_tiles = p3.n_tiles;
-    g3.out_cols = out_cols;
-    g3.use_res_tma = d->residual ? 1 : 0;
-    g3.ln_stats = d->ln_stats, g3.ln_parts = d->ln_parts, g3.ln_eps = d->ln_eps, g3.ln_colsum = d->ln_colsum;
-    g3.ln_inv_c = 1.0f / (float)(d->c0 + d->c1);
-    g3.stats_out = d->stats_out;
-    {
-      const long long total_tiles = (long long)p3.m_groups * p3.n_tiles + num_sms();  // the epilogue also locates one tile past the end
-      const long long dmax = std::max(p3.m_groups, std::max(p3.tiles_w, p3.tiles_h));
-      if (total_tiles * dmax >= (1LL << 32) || (long long)(p3.m_groups * p3.ctas + 1) * dmax >= (1LL << 32))
-        return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: tile grid too large for the 32-bit tile decomposition");
-      g3.mg_magic = div_magic(p3.m_groups), g3.tw_magic = div_magic(p3.tiles_w), g3.th_magic = div_magic(p3.tiles_h);
-    }
-    return kernel == 2 ? launch3_bn<2>(p3, tA0, tA1, tB, tO, tR, g3, st) : launch3_bn<1>(p3, tA0, tA1, tB, tO, tR, g3, st);
-  }
 
   CUtensorMap tA0, tA1, tB;
   if (!make_act_map(&tA0, d->a0, d->c0, d->lda0, d->n_img, d->h_in, d->w_in, pl.bn, pl.bh, pl.bw, d->stride))
@@ -398,7 +247,7 @@ extern "C" int mdb_gemm_conv(const mdb_gemm_desc* d, void* stream) {
     tA1 = tA0;
   }
   const int ktot = d->taps_h * d->taps_w * (d->c0 + d->c1);
-  if (!make_w_map(&tB, d->w, d->n_out, ktot, pl.block_n))
+  if (!make_w_map(&tB, d->w, d->n_out, ktot, pl.block_n / pl.ctas))
     return set_error(MDB_ERR_CUDA, "cuTensorMapEncodeTiled(W) failed (n=%d k=%d)", d->n_out, ktot);
 
   GemmParams gp;
@@ -407,6 +256,8 @@ extern "C" int mdb_gemm_conv(const mdb_gemm_desc* d, void* stream) {
   gp.taps_h = d->taps_h, gp.taps_w = d->taps_w, gp.stride = d->stride, gp.pad_h = d->pad_h, gp.pad_w = d->pad_w;
   gp.cblocks0 = d->c0 / 64, gp.cblocks1 = d->c1 / 64;
   gp.bn = pl.bn, gp.bh = pl.bh, gp.bw = pl.bw, gp.tiles_h = pl.tiles_h, gp.tiles_w = pl.tiles_w;
+  gp.m_tiles = pl.tiles_n * pl.tiles_h * pl.tiles_w, gp.n_tiles = pl.n_tiles, gp.splits = pl.splits;
+  gp.m_groups = pl.m_groups;
   gp.kb_per_split = pl.kb_per_split;
   gp.epi_mode = pl.splits > 1 ? EPI_PARTIAL_F32 : d->epi_mode;
   gp.out_is_f32 = d->out_is_f32;
@@ -414,16 +265,11 @@ extern "C" int mdb_gemm_conv(const mdb_gemm_desc* d, void* stream) {
   gp.residual = static_cast<const __nv_bfloat16*>(d->residual), gp.ldr = d->ldr;
   gp.out = d->out, gp.ldo = d->ldo, gp.out_scale = d->out_scale;
   gp.partial = static_cast<float*>(d->workspace);
-  gp.trace = static_cast<long long*>(d->trace);
-  gp.debug_flags = d->debug_flags;
+  gp.ln_stats = d->ln_stats, gp.ln_parts = d->ln_parts, gp.ln_eps = d->ln_eps, gp.ln_colsum = d->ln_colsum;
+  gp.ln_inv_c = 1.0f / (float)(d->c0 + d->c1);
+  gp.stats_out = d->stats_out;
 
-  switch (pl.block_n) {
-    case 256: rc = launch2<256>(pl, tA0, tA1, tB, gp, st); break;
-    case 160: rc = launch2<160>(pl, tA0, tA1, tB, gp, st); break;
-    case 128: rc = launch2<128>(pl, tA0, tA1, tB, gp, st); break;
-    case 64: rc = launch2<64>(pl, tA0, tA1, tB, gp, st); break;
-    default: return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: unsupported block_n %d", pl.block_n);
-  }
+  rc = pl.ctas == 2 ? launch_bn<2>(pl.block_n, tA0, tA1, tB, gp, st) : launch_bn<1>(pl.block_n, tA0, tA1, tB, gp, st);
   if (rc != MDB_OK) return rc;
   if (pl.splits > 1) {
     const long long pixels = (long long)d->n_img * d->h_out * d->w_out;

@@ -8,10 +8,9 @@
 #include "common_host.h"
 #include "ptx_cluster.cuh"
 
-// Images of at least this many bytes take the pixel-major cluster GroupNorm when MDB_GN_ROWS is unset: measured crossover
-// against gn_fused_kernel on B200 (tools/bench_norm.py, profiles/gn_rows_r2.txt) -- 12 x 1400 x 320: 16.5 vs 21.4 us,
-// 12 x 350 x 1920: 20.5 vs 22.6 us, equal at 12 x 350 x 1280, slower below; inputs that only fit a 16-CTA cluster win from
-// 2.5 MB (12 x 1400 x 960: 39.0 vs 43.8 us; 12 x 1400 x 640 loses 30.9 vs 28.7 us).
+// Images of at least this many bytes take the pixel-major cluster GroupNorm when MDB_GN_ROWS is unset (the crossover against
+// gn_fused_kernel; a larger threshold for inputs that only fit a 16-CTA cluster).  tools/bench_norm.py times both kernels on
+// the shapes of one denoising step.
 #ifndef MDB_GN_ROWS_MIN_BYTES
 #define MDB_GN_ROWS_MIN_BYTES 850000LL
 #endif
@@ -478,7 +477,7 @@ extern "C" int mdb_groupnorm(const void* x0, int c0, int ld0, const void* x1, in
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   {
     // pixel-major cluster kernel: the default wherever an image is large enough that gn_fused_kernel's channel-slice reads
-    // cost more than the cluster barrier (measured crossover, profiles/); MDB_GN_ROWS=1 forces it, =0 disables it
+    // cost more than the cluster barrier (MDB_GN_ROWS_MIN_BYTES); MDB_GN_ROWS=1 forces it, =0 disables it
     const char* env = getenv("MDB_GN_ROWS");  // read per call: tests flip it inside one process
     const int mode = env ? ((env[0] == '1') ? 1 : 0) : -1;
     const int vpp = ctot / 8;
@@ -574,7 +573,13 @@ extern "C" int mdb_groupnorm(const void* x0, int c0, int ld0, const void* x1, in
   if (R > 16) R = 16;
   const int threads = vpp * R;  // <= 512
   // enough CTAs to fill the machine: ~4 per SM over all images
-  int chunks = (148 * 4 + n_img - 1) / n_img;
+  static int sms = 0;
+  if (!sms) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
+  }
+  int chunks = (sms * 4 + n_img - 1) / n_img;
   int pix_per_cta = (hw + chunks - 1) / chunks;
   if (pix_per_cta < R) pix_per_cta = R;
   chunks = (hw + pix_per_cta - 1) / pix_per_cta;

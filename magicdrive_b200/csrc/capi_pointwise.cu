@@ -219,8 +219,7 @@ __global__ void linear_small_kernel(const float* __restrict__ in, int m, int k, 
 
 // Direct convolution, one thread per output element (output channel fastest), fp32 accumulate.  Weights are [kh][kw][cin][cout]:
 // the threads of a warp (consecutive output channels of one pixel) read consecutive weights and broadcast-read the same input
-// value.  (With [cout][kh][kw][cin] weights every lane walked its own row, 32 sectors per load: the BEV-map encoder took
-// 12.9 ms of the 15.3 ms a re-conditioning call costs, profiles/time_prepare_r2.txt.)
+// value.  (With [cout][kh][kw][cin] weights every lane would walk its own row: 32 sectors per load.)
 template <typename TI>
 __global__ void conv_direct_kernel(const TI* __restrict__ x, int n, int h, int w, int cin, const float* __restrict__ wgt,
                                    const float* __restrict__ bias, int cout, int kh, int kw, int sh, int sw, int ph,

@@ -1,5 +1,6 @@
-// Operand scheme and shared definitions of the tcgen05 GEMM / implicit-GEMM convolution kernels for sm_100a
-// (gemm_tc2.cuh: single-CTA persistent kernel with split-K; gemm_pair.cuh: CTA-pair kernel with the TMA-store epilogue).
+// Operand scheme and shared definitions of the tensor-core GEMM / implicit-GEMM convolution for sm_90a
+// (gemm_wgmma.cuh: persistent warp-specialised kernel, TMA producer + two wgmma consumer warpgroups, on single CTAs
+// with split-K or on 2-CTA clusters that share each weight tile through TMA multicast).
 //
 //   D[pixel, n] = sum_{tap, c}  A[pixel shifted by tap, c] * W[n, tap*C + c]      (+ epilogue)
 //
@@ -10,8 +11,8 @@
 //   Two A sources are supported (the K loop runs over source 0's channels then source 1's): this is how
 //   channel-concatenated inputs (UNet skip connections) are consumed without materialising the concat.
 // * W is a bf16 [N, K] (K-major) matrix behind a 2-D tensor map, K ordered (tap, channel).
-// * Both operands land in shared memory with the 128-byte swizzle and are consumed by tcgen05.mma
-//   (M=128, N=BLOCK_N, K=16, bf16 x bf16 -> fp32 in TMEM).
+// * Both operands land in shared memory with the 128-byte swizzle and are consumed by wgmma
+//   (per consumer warpgroup M=64, N=BLOCK_N, K=16, bf16 x bf16 -> fp32 in registers).
 #pragma once
 #include "ptx.cuh"
 
@@ -28,8 +29,9 @@ struct GemmParams {
   int cblocks0, cblocks1;  // 64-channel blocks of A source 0 / 1
   // M-tile box
   int bn, bh, bw;
-  int tiles_h, tiles_w;  // tiles per image column/row direction (tiles over images = gridDim.x / (tiles_h*tiles_w))
-  // split-K
+  int tiles_h, tiles_w;  // tiles per image column/row direction
+  int m_tiles, n_tiles, splits;  // tiles = m_tiles * n_tiles * splits (m fastest)
+  int m_groups;                  // ceil(m_tiles / CTAS): M tiles are walked in groups of one per CTA of a cluster
   int kb_per_split;
   // epilogue
   int epi_mode;
@@ -43,8 +45,13 @@ struct GemmParams {
   int ldo;
   float out_scale;
   float* partial;  // [splits][pixels][n_out] fp32 workspace (EPI_PARTIAL_F32)
-  int debug_flags;   // debug/ablation: 1 = skip output stores, 2 = skip bias/shift/residual loads, 4 = skip TMEM loads
-  long long* trace;  // optional debug: per-CTA clock64 stamps (16 slots per CTA, first 8 CTAs)
+  // LayerNorm folded into this GEMM (consumer side): out = rstd * scale * (acc - mean * colsum_n) + c_n
+  const float* ln_stats;   // [pixels][ln_parts][2] partial (sum, sum sq) of the A rows, or nullptr
+  int ln_parts;
+  float ln_inv_c, ln_eps;
+  const float* ln_colsum;  // [n_out] sum_k W'[n, k]
+  // row statistics of this GEMM's output (producer side): [pixels][n_tiles][2] partial (sum, sum sq), or nullptr
+  float* stats_out;
 };
 
 constexpr int kBlockM = 128;

@@ -1,9 +1,5 @@
-// Inline-PTX wrappers for the CTA-pair (cta_group::2) form of tcgen05 and for TMA stores (sm_100a).
-//   * a CTA pair is a 2-CTA cluster on one TPC; tcgen05.mma.cta_group::2 is issued by the rank-0 ("leader") CTA and
-//     consumes the A rows / B columns staged in BOTH CTAs' shared memory, writing 128 accumulator rows into each
-//     CTA's own TMEM;
-//   * both CTAs' TMA loads complete on the LEADER's mbarrier (its shared::cluster address), the MMA's commit is
-//     multicast to the same barrier offset in both CTAs;
+// Inline-PTX wrappers for thread-block clusters and bulk copies (sm_90a):
+//   * cluster rank / barriers and distributed-shared-memory addressing (mapa), remote mbarrier arrive;
 //   * TMA stores (cp.async.bulk.tensor ... global.shared::cta) drain a shared-memory box to global memory without
 //     using the LSU; bulk async-groups are per thread.
 #pragma once
@@ -33,53 +29,18 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t local_smem_addr, uint32_t 
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
   asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
-
-// ---------------------------------------------------------------- TMEM, pair form (one warp of EACH CTA executes these)
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
+// the same with release semantics at cluster scope: everything this thread did before is visible to the waiting CTA
+__device__ __forceinline__ void mbar_arrive_cluster_release(uint32_t cluster_addr) {
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
-__device__ __forceinline__ void tmem_relinquish_pair() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// D[tmem of both CTAs] (+)= A[smem of both CTAs: 256 rows] * B[smem of both CTAs: N columns]; issued by the leader CTA.
-__device__ __forceinline__ void umma_bf16_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                               uint32_t accumulate) {
+// TMA load of one box, written to the same shared-memory offset in every CTA of `mask`; each destination CTA's mbarrier at
+// the offset of `bar` receives the bytes that land in it
+__device__ __forceinline__ void tma_load_2d_multicast(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1,
+                                                      uint16_t mask) {
   asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive (once all MMAs issued so far have completed) on the mbarrier at this shared-memory offset in every CTA of `mask`.
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(mask)
-               : "memory");
-}
-
-// ---------------------------------------------------------------- TMA loads whose completion lands on another CTA's barrier
-__device__ __forceinline__ void tma_load_2d_pair(const CUtensorMap* m, uint32_t bar_cluster_addr, void* dst, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair(const CUtensorMap* m, uint32_t bar_cluster_addr, void* dst, int c0, int c1,
-                                                 int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(dst)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
       : "memory");
 }
 

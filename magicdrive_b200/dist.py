@@ -60,7 +60,7 @@ def gather_scenes(local: torch.Tensor, n_total: int) -> torch.Tensor:
 def shutdown(denoisers=(), timeout_s: float = 20.0, exit_code: int = 0, hard_exit_on_timeout: bool = True) -> None:
     """Tear the process group down at the end of a run.  A CUDA graph that captured NCCL collectives (view-sharded mode)
     keeps the communicator busy: release the graphs first; if the communicator still does not come down within
-    `timeout_s` (observed on 2 x B200, NCCL 2.28.9: destroy_process_group never returned with a live graph), warn, flush
+    `timeout_s` (observed with NCCL 2.28.9: destroy_process_group never returned with a live graph), warn, flush
     and leave the process with `exit_code` (the status the caller would have returned) without running the remaining
     teardown; with hard_exit_on_timeout=False the caller gets control back instead."""
     for d in denoisers:

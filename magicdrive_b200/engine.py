@@ -1,6 +1,6 @@
 """CUDA execution of the two hot-path networks over the C-ABI operators (magicdrive_b200.ops).
 
-Dataflow differs from the reference on purpose (B200-first), results do not:
+Dataflow differs from the reference on purpose (GPU-first), results do not:
   * activations are bf16 NHWC == [tokens, C]: the NCHW<->token permutes of Transformer2DModel
     (transformer_2d.py:286,305) and the 1x1-conv / Linear distinction vanish;
   * skip-connection concats (unet_2d_blocks.py:1984,2086) are never materialised: GroupNorm and the convolutions

@@ -4,7 +4,7 @@
 (so `load_state_dict(reference.state_dict())` and the diffusers `save_pretrained` directories load unchanged),
 `forward` signatures and return types (magicdrive/networks/unet_2d_condition_multiview.py:327-339,524-527;
 magicdrive/networks/unet_addon_rawbox.py:707-724,921-932), plus the helper methods the pipeline calls
-(`uncond_cam_param`, `add_uncond_to_kwargs`, `prepare`).  Their arithmetic runs in `engine.py` on the sm_100a
+(`uncond_cam_param`, `add_uncond_to_kwargs`, `prepare`).  Their arithmetic runs in `engine.py` on the sm_90a
 kernels; inputs must be CUDA tensors — there is no CPU path (ops raise).
 """
 import json
@@ -129,7 +129,7 @@ class _B200Module(nn.Module):
     def _get_engine(self, cls_):
         dev = self.device
         if dev.type != "cuda":
-            raise ops._lib.MdbError(f"{type(self).__name__} runs only on a CUDA (sm_100a) device; parameters are on {dev}")
+            raise ops._lib.MdbError(f"{type(self).__name__} runs only on a CUDA (sm_90a) device; parameters are on {dev}")
         if self._engine is None:
             self._engine = cls_(self.arch_cfg, dict(self.state_dict()), dev)
             if self._view_shard is not None and hasattr(self._engine, "set_view_shard"):
@@ -162,7 +162,7 @@ def _pick(cfg_cls, kwargs):
 
 
 class UNet2DConditionModelMultiview(_B200Module):
-    """B200-native stand-in for magicdrive.networks.unet_2d_condition_multiview.UNet2DConditionModelMultiview."""
+    """CUDA-native stand-in for magicdrive.networks.unet_2d_condition_multiview.UNet2DConditionModelMultiview."""
 
     def __init__(self, **kwargs):
         super().__init__()
@@ -177,7 +177,7 @@ class UNet2DConditionModelMultiview(_B200Module):
                         ("upcast_attention", False), ("center_input_sample", False), ("encoder_hid_dim", None),
                         ("crossview_attn_type", "basic"), ("only_cross_attention", False), ("act_fn", "silu")):
             if extra.get(k, want) != want:
-                raise ValueError(f"UNet2DConditionModelMultiview (B200): unsupported config {k}={extra[k]!r}")
+                raise ValueError(f"UNet2DConditionModelMultiview (CUDA): unsupported config {k}={extra[k]!r}")
         self._init_common(cfg, arch.unet_param_shapes(cfg), extra)
 
     @classmethod
@@ -230,7 +230,7 @@ class UNet2DConditionModelMultiview(_B200Module):
 
 
 class BEVControlNetModel(_B200Module):
-    """B200-native stand-in for magicdrive.networks.unet_addon_rawbox.BEVControlNetModel (inference path)."""
+    """CUDA-native stand-in for magicdrive.networks.unet_addon_rawbox.BEVControlNetModel (inference path)."""
 
     def __init__(self, **kwargs):
         super().__init__()

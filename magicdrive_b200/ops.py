@@ -20,7 +20,7 @@ from ._lib import GemmDesc, check
 BF16 = torch.bfloat16
 F32 = torch.float32
 
-GEMM_VARIANT = int(os.environ.get('MDB_GEMM_VARIANT', '0'))  # A/B hook: mdb_gemm_desc.kernel_variant (2 = single-CTA kernel, 3 = CTA pairs)
+GEMM_VARIANT = int(os.environ.get('MDB_GEMM_VARIANT', '0'))  # A/B hook: mdb_gemm_desc.kernel_variant (2 = single CTAs, 3 = CTA pairs)
 _launches = 0  # kernels launched through this module (bench.py reports it as gpu_launches)
 _profile = None  # when a list: (kind, algorithmic flops, start event, end event) per tensor-core launch
 
@@ -124,11 +124,10 @@ def gemm_conv(a0: torch.Tensor, w: torch.Tensor, *, n_img: int, h_in: int, w_in:
               bias: Optional[torch.Tensor] = None, rowbias: Optional[torch.Tensor] = None,
               residual: Optional[torch.Tensor] = None, ldr: int = 0, out: Optional[torch.Tensor] = None,
               ldo: Optional[int] = None, out_f32: bool = False, out_scale: float = 1.0, geglu: bool = False,
-              force_block_n: int = 0, force_splits: int = 0, allow_split_k: bool = True,
-              kernel_variant: int = 0, trace: Optional[torch.Tensor] = None, debug_flags: int = 0,
+              force_block_n: int = 0, force_splits: int = 0, allow_split_k: bool = True, kernel_variant: int = 0,
               ln: Optional["RowStats"] = None, ln_colsum: Optional[torch.Tensor] = None, ln_eps: float = 1e-5,
               emit_stats: bool = False):
-    """tcgen05 GEMM / implicit-GEMM conv (mdb_gemm_conv).  `a0` (and `a1`) are NHWC bf16 buffers whose pixel
+    """wgmma GEMM / implicit-GEMM conv (mdb_gemm_conv).  `a0` (and `a1`) are NHWC bf16 buffers whose pixel
     stride is lda* elements; `w` is bf16 [n_out, taps*taps*(c0+c1)].
     ln / ln_colsum: fold a LayerNorm of the rows of `a0` into this GEMM (`ln` = the RowStats the producer of `a0`
     emitted, `w` pre-multiplied by gamma, `bias` = beta-term + bias).  emit_stats: also return the RowStats of the
@@ -167,8 +166,6 @@ def gemm_conv(a0: torch.Tensor, w: torch.Tensor, *, n_img: int, h_in: int, w_in:
         d.workspace, d.workspace_bytes = None, 0
     d.force_block_n, d.force_splits = force_block_n, force_splits
     d.kernel_variant = kernel_variant or GEMM_VARIANT
-    d.trace = _ptr(trace)
-    d.debug_flags = debug_flags
     L = _lib.lib()
     if ln is not None:
         d.ln_stats, d.ln_parts, d.ln_eps, d.ln_colsum = ln.data.data_ptr(), ln.parts, float(ln_eps), _ptr(ln_colsum)

@@ -1,4 +1,4 @@
-"""Weight packing for the sm_100a kernels (bf16, K-major, tap-major conv filters, GEGLU tile interleave)."""
+"""Weight packing for the sm_90a kernels (bf16, K-major, tap-major conv filters, GEGLU tile interleave)."""
 import torch
 
 

@@ -1,5 +1,5 @@
 """The denoising loop of StableDiffusionBEVControlNetPipeline.__call__ (magicdrive/pipeline/pipeline_bev_controlnet.py:
-303-451) on top of the B200 engines: classifier-free-guidance batching ([uncond ; cond]), ControlNet -> UNet ->
+303-451) on top of the CUDA engines: classifier-free-guidance batching ([uncond ; cond]), ControlNet -> UNet ->
 guidance -> DDIM update per step, with everything step-invariant hoisted and one whole step captured in a CUDA graph.
 
 Differences from the reference that do not change results: latents stay fp32 and NHWC-resident between steps

@@ -11,6 +11,7 @@ import torch
 
 from magicdrive_b200 import arch
 from oracle import ref_shim
+from tests.common import save_golden
 
 OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden")
 
@@ -52,9 +53,8 @@ def main():
     eps = mv(lat5.reshape(-1, 4, h, w), t[0], encoder_hidden_states=ctx, down_block_additional_residuals=down,
              mid_block_additional_residual=mid).sample
     eps_noctrl = mv(lat5.reshape(-1, 4, h, w), t[0], encoder_hidden_states=ctx).sample
-    torch.save(dict(inputs=inp, t=481, down=[d.clone() for d in down], mid=mid, ctx=ctx, eps=eps,
-                    eps_noctrl=eps_noctrl, seed=7, shape=(scenes, n_cam, h, w)),
-               os.path.join(OUT, "tiny_forward.pt"))
+    save_golden(dict(inputs=inp, t=481, down=[d.clone() for d in down], mid=mid, ctx=ctx, eps=eps,
+                     eps_noctrl=eps_noctrl, seed=7, shape=(scenes, n_cam, h, w)), "tiny_forward.pt")
 
     # ---- golden 2: the reference pipeline loop (CFG 2.0, 3 DDIM steps, boxes + map)
     R = ref_shim.load()

@@ -31,7 +31,7 @@ def main():
         print(at, out["eps"][at].shape, float(out["eps"][at].abs().mean()))
     # ControlNet with guess_mode=True, conditioning_scale 0.7 (unet_addon_rawbox.py:897-905): inputs of tiny_forward.pt
     from oracle.make_golden import load_ref
-    from tests.common import golden
+    from tests.common import golden, save_golden
     gf = golden("tiny_forward.pt")
     _, cn, _, _ = load_ref(ucfg0, ccfg, seed=gf["seed"])
     inp = gf["inputs"]
@@ -53,7 +53,7 @@ def main():
                        return_dict=False)
     out["map_plus"] = dict(seed=seed + 1, bev_map=bev, embedding=emb.clone(), mid=mid.clone(), down0=down[0].clone(),
                            inputs_from="tiny_forward.pt")
-    torch.save(out, os.path.join(OUT, "tiny_attn_types.pt"))
+    save_golden(out, "tiny_attn_types.pt")
 
 
 if __name__ == "__main__":

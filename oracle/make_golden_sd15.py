@@ -5,7 +5,7 @@ configuration the benchmark times (4 levels, head dims 40 / 80 / 160, 6 views, 2
 
     python -m oracle.make_golden_sd15       # build container (needs /root/reference or the oracle/_ref snapshot), ~3 min
 
-Stored (tests/golden/sd15_forward.pt, ~1.4 MB): the predicted noise in full; the mid residual, ControlNet residuals 0 and 11
+Stored (tests/golden/sd15_forward.pt + sd15_forward.down0.pt): the predicted noise in full; the mid residual, ControlNet residuals 0 and 11
 and the conditioning tokens on a fixed channel subset (every 16th / 8th channel), enough to pin a structural error anywhere
 on the path without committing 40 MB of activations.  The oracle (tests/test_oracle_cpu.py) and the CUDA path
 (tests/test_model_gpu.py) are both checked against it.
@@ -18,6 +18,7 @@ import torch
 from magicdrive_b200 import arch
 from magicdrive_b200.synthetic import synthetic_inputs
 from oracle import ref_shim
+from tests.common import save_golden
 
 OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden", "sd15_forward.pt")
 SEEDS = (11, 12)
@@ -38,11 +39,11 @@ def main():
                         return_dict=False)
     eps = mv(lat5.reshape(-1, 4, H, W), t[0], encoder_hidden_states=ctx, down_block_additional_residuals=down,
              mid_block_additional_residual=mid).sample
-    torch.save(dict(seeds=SEEDS, input_seed=INPUT_SEED, t=T, shape=(1, 6, H, W), n_box=N_BOX, map_hw=MAP_HW,
+    save_golden(dict(seeds=SEEDS, input_seed=INPUT_SEED, t=T, shape=(1, 6, H, W), n_box=N_BOX, map_hw=MAP_HW,
                     ch_step=CH_STEP, ctx_step=CTX_STEP, eps=eps.clone(), mid=mid[:, ::CH_STEP].clone(),
                     down0=down[0][:, ::CH_STEP].clone(), down11=down[11][:, ::CH_STEP].clone(),
                     ctx=ctx[:, :, ::CTX_STEP].clone(), n_down=len(down),
-                    down_norms=[float(d.norm()) for d in down]), OUT)
+                    down_norms=[float(d.norm()) for d in down]), os.path.basename(OUT))
     print(OUT, os.path.getsize(OUT) // 1024, "KiB; eps", tuple(eps.shape), "|eps|", float(eps.norm()))
 
 

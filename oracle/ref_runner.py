@@ -3,7 +3,7 @@ own UNet2DConditionModelMultiview + BEVControlNetModel, loaded through oracle/re
 oracle/_ref snapshot) on this repo's synthetic workload, and time its denoising steps.
 
 Used by `bench.py --impl reference` (CPU, fp32: the reference arm), by bench.py's `gpu_reference` field (same GPU, bf16,
-diffusers' AttnProcessor2_0 = torch SDPA, since the vendored xformers cannot run on sm_100: SURVEY.md section 0.4) and by
+diffusers' AttnProcessor2_0 = torch SDPA, since the vendored xformers only dispatches below compute capability 9.0: SURVEY.md section 0.4) and by
 tests.  The product never imports this module.
 """
 import time

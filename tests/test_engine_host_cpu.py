@@ -310,8 +310,8 @@ def test_full_sd15_width_engines_through_emulated_operators(emulated):
 def test_bf16_storage_alone_accounts_for_the_gpu_parity_gap(emulated, monkeypatch):
     """With the operator restatements rounding every activation to bf16 exactly where the device stores one (fp32
     arithmetic otherwise), the 3-step CFG pipeline lands 8.4e-3 (rel-L2) from the reference fixture — the same distance the
-    CUDA path measures on a B200 (profiles/parity_r1.txt: 8.2e-3 .. 8.4e-3).  The GPU tolerance (2e-2) is therefore a
-    statement about bf16 storage, not slack for kernel error."""
+    CUDA path measures on an H100 (tests/test_model_gpu.py, pipeline parity: 8.3e-3).  The GPU tolerance (2e-2) is therefore
+    a statement about bf16 storage, not slack for kernel error."""
     from tests.common import golden, tiny_state_dicts
     monkeypatch.setattr(ops_emulator, "ROUND_ACTIVATIONS", True)
     p = golden("tiny_pipeline.pt")

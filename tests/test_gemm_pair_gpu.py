@@ -1,6 +1,7 @@
-"""GPU parity of gemm_pair_kernel (CTA-pair tcgen05 GEMM / implicit-GEMM conv, TMA-store epilogue, folded LayerNorm)
-against plain torch fp32 on the same bf16-rounded inputs.  kernel_variant 3 = CTA pairs (cta_group::2), 4 = the same
-kernel on single CTAs, 2 = the previous single-CTA kernel (yardstick: both must agree with torch equally well)."""
+"""GPU parity of the wgmma GEMM / implicit-GEMM conv with bf16 output (bias / per-image shift / residual / scale, GEGLU,
+row statistics, folded LayerNorm) against plain torch fp32 on the same bf16-rounded inputs.  kernel_variant 3 = CTA pairs
+(2-CTA clusters sharing each weight tile through TMA multicast), 4 = the same kernel on single CTAs without split-K,
+2 = single CTAs with split-K allowed (yardstick: all must agree with torch equally well)."""
 import math
 
 import pytest
@@ -117,7 +118,7 @@ def test_conv3x3(cuda_lib, n, h, w, ci, co, stride, variant):
 
 @pytest.mark.parametrize("variant", VARIANTS, ids=VARIANT_IDS)
 def test_conv3x3_small_images_many_per_tile(cuda_lib, variant):
-    """4x7 level: several images per 128-row tile; without a per-image shift the pair kernel must handle it."""
+    """4x7 level: several images per 128-row tile (and, for pairs, a cluster whose second tile lies past the last image)."""
     g = torch.Generator(device="cuda").manual_seed(8)
     n, h, w, ci, co = 5, 4, 7, 1280, 1280
     x = _bf(torch.randn(n, ci, h, w, device="cuda", generator=g))

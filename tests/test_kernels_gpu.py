@@ -28,7 +28,7 @@ def _conv_weight(wt):  # [co, ci, kh, kw] -> [co, kh*kw*ci] (tap-major, channel-
     return wt.permute(0, 2, 3, 1).reshape(co, kh * kw * ci).contiguous()
 
 
-@pytest.mark.parametrize("variant", [0, 2])  # 0 = planner's choice (CTA-pair kernel where it applies), 2 = single-CTA persistent kernel
+@pytest.mark.parametrize("variant", [0, 2])  # 0 = planner's choice, 2 = single CTAs
 @pytest.mark.parametrize("bn", [0, 64, 128, 160, 256])
 @pytest.mark.parametrize("m,k,n", [(1000, 320, 320), (128, 64, 640), (336, 1280, 1280), (16800, 320, 960)])
 def test_gemm_plain(cuda_lib, bn, m, k, n, variant):
@@ -187,7 +187,7 @@ def test_layernorm(cuda_lib, c):
     assert _rel(out, ref) < 8e-3
 
 
-ATTN_KERNELS = ["tc2", "tc2d", "tc"]  # tcgen05 v2 (2 CTAs/SM | double-buffered S; d = 160 falls to tc), tcgen05 v1
+ATTN_KERNELS = ["tc2", "tc2d", "tc"]  # key-tile width: per head dim (default) | 64 keys | 128 keys
 
 
 def _pick_attention_kernel(monkeypatch, kernel):
@@ -220,8 +220,8 @@ def test_attention(cuda_lib, monkeypatch, d, heads, lq, lk, kernel):
 @pytest.mark.parametrize("b,heads,d,lq,lk", [(12, 8, 40, 1400, 98), (12, 8, 40, 1337, 128), (12, 8, 40, 1400, 40), (30, 2, 32, 1400, 77),
                                              (30, 2, 64, 700, 98), (40, 8, 40, 300, 1)])
 def test_attention_multi_q_tiles_per_cta(cuda_lib, monkeypatch, b, heads, d, lq, lk):
-    """One K/V tile (lk <= 128) and more query tiles than CTA slots: the single-S kernel's multi-Q instantiation (a CTA keeps the
-    K/V tile and walks several query tiles) against fp32 torch and, bit for bit, against the one-tile-per-CTA kernel."""
+    """One K/V tile (lk <= 128) and more query tiles than CTA slots: multi-Q mode (a CTA keeps the K/V tile and walks several
+    query tiles) against fp32 torch and, bit for bit, against one query tile per CTA."""
     monkeypatch.delenv("MDB_ATTN_KERNEL", raising=False)
     g = torch.Generator(device="cuda").manual_seed(29)
     c = heads * d
@@ -246,7 +246,7 @@ def test_attention_multi_q_tiles_per_cta(cuda_lib, monkeypatch, b, heads, d, lq,
 @pytest.mark.parametrize("lq,lk", [(300, 700), (1400, 1400)])
 def test_attention_growing_scores(cuda_lib, monkeypatch, d, heads, lq, lk, kernel):
     """Scores that grow along the key axis (later key tiles dominate by far more than 2^8): exercises the running-max
-    update of the online softmax, incl. the in-TMEM accumulator rescale of the tc2 kernel."""
+    update of the online softmax and the rescale of the running output accumulator."""
     _pick_attention_kernel(monkeypatch, kernel)
     g = torch.Generator(device="cuda").manual_seed(19)
     b = 2

@@ -5,7 +5,7 @@ Tolerance: bf16 storage cannot meet rtol 1e-3 / atol 1e-4 elementwise (the refer
 its fp32 forward by more, SURVEY.md section 7 "Tolerance"; the fp32 oracle does meet it literally against the reference at full
 size, tests/test_oracle_cpu.py); the criterion is  err(ours-bf16 vs fp32 truth) <= 1.0 x err(reference-arithmetic-in-bf16 vs
 fp32 truth) + 5e-4  at every tap, where "reference arithmetic in bf16" is the oracle restatement run with bf16
-weights/activations through torch's own CUDA kernels.  Every measured number is appended to profiles/parity_gpu_latest.txt."""
+weights/activations through torch's own CUDA kernels.  Every measured number is printed (tests.common.record)."""
 import os
 from dataclasses import asdict
 
@@ -259,7 +259,7 @@ def test_view_sharded_cross_view_attention_two_gpus():
     import subprocess
     import sys
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 visible GPUs (spawns torchrun; last run: profiles/view_shard_r1.txt)")
+        pytest.skip("needs 2 visible GPUs (spawns torchrun)")
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2",
                         "--master-addr", "127.0.0.1", "--master-port", "29611", os.path.join(root, "tools", "check_view_shard.py")],

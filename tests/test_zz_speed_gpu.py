@@ -1,8 +1,8 @@
 """GPU-reference timing (SURVEY.md §8d-i): the reference's arithmetic for one CFG scene-step -- the oracle restatement
 in bf16 on torch's own CUDA kernels (cuDNN convolutions, cuBLAS GEMMs, F.scaled_dot_product_attention like the reference's
 AttnProcessor2_0) -- timed on the same GPU next to this repo's path.  The reference itself cannot travel to the GPU box
-and its vendored xformers does not run on sm_100 (SURVEY.md §0.4), so this is the stand-in for "the reference's CUDA
-path on 1xB200".  Named test_zz_* so that it runs after the parity tests; the oracle is only the thing compared with."""
+and its vendored xformers only dispatches below compute capability 9.0 (SURVEY.md §0.4), so this is the stand-in for
+"the reference's CUDA path on 1xH100".  Named test_zz_* so that it runs after the parity tests; the oracle is only the thing compared with."""
 import sys
 import os
 from dataclasses import asdict

@@ -9,7 +9,7 @@ pids=()
 for f in $root/magicdrive_b200/csrc/*.cu; do
   b=$(basename $f .cu)
   fm="--use_fast_math"; case $b in capi_pointwise|capi_gemm|capi_inputprep) fm="";; esac
-  nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC $fm "$@" -c $f -o $out/$name/$b.o 2>/dev/null &
+  nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC $fm "$@" -c $f -o $out/$name/$b.o 2>/dev/null &
   pids+=($!)
 done
 for p in "${pids[@]}"; do wait $p; done
