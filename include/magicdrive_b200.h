@@ -94,6 +94,9 @@ int mdb_gemm_conv_launches(const mdb_gemm_desc* d);
 /* Partial-sum slots per output row that mdb_gemm_conv writes to stats_out for this descriptor (depends on the tiling the
  * planner picks); negative status if the descriptor cannot emit row statistics. */
 int mdb_gemm_conv_stats_parts(const mdb_gemm_desc* d);
+/* The planner's tiling for this descriptor, for profiling tools: plan[0..4] = block_n, M tiles, N tiles, K splits,
+ * waves of the persistent grid. */
+int mdb_gemm_conv_plan(const mdb_gemm_desc* d, int* plan);
 
 /* Direct (CUDA-core) convolution for tiny channel counts: conv_in 4->320 (unet_2d_condition.py:231),
  * conv_out 320->4 (:503), BEV map encoder (magicdrive/networks/map_embedder.py:66-76).

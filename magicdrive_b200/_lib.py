@@ -44,6 +44,7 @@ SIGNATURES = {
     "mdb_gemm_conv": (_i, [C.POINTER(GemmDesc), _vp]),
     "mdb_gemm_conv_launches": (_i, [C.POINTER(GemmDesc)]),
     "mdb_gemm_conv_stats_parts": (_i, [C.POINTER(GemmDesc)]),
+    "mdb_gemm_conv_plan": (_i, [C.POINTER(GemmDesc), C.POINTER(C.c_int)]),
     "mdb_conv_direct": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp]),
     "mdb_groupnorm": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp, _i, _vp, _i, _vp, _vp]),
     "mdb_layernorm": (_i, [_vp, _ll, _i, _i, _vp, _vp, _f, _vp, _i, _vp]),

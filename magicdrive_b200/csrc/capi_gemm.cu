@@ -16,19 +16,41 @@ using namespace mdb;
 
 namespace {
 
-// 4-D activation map: dims (C, W, H, N) innermost first; pixel stride = ld elements.
-bool make_act_map(CUtensorMap* m, const void* ptr, int c, int ld, int n, int h, int w, int bn, int bh, int bw,
-                  int stride) {
-  EncodeTiledFn enc = get_encode();
+// A operand of a convolution: 4-D (C, W, H, N) im2col map, innermost first; pixel stride = ld elements.  The bounding box
+// of filter-tap-(0, 0) positions runs from -pad to (extent - 1 + pad - (taps - 1)) in each spatial dimension, walked with
+// the stride: exactly h_out x w_out positions per image.
+bool make_im2col_map(CUtensorMap* m, const void* ptr, int c, int ld, const mdb_gemm_desc* d) {
+  EncodeIm2colFn enc = get_encode_im2col();
   if (!enc) return false;
+  const int n = d->n_img, h = d->h_in, w = d->w_in;
   cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
   cuuint64_t strides[3] = {(cuuint64_t)ld * 2, (cuuint64_t)w * ld * 2, (cuuint64_t)h * w * ld * 2};
-  cuuint32_t box[4] = {64u, (cuuint32_t)(bw * stride), (cuuint32_t)(bh * stride), (cuuint32_t)bn};
-  cuuint32_t estr[4] = {1u, (cuuint32_t)stride, (cuuint32_t)stride, 1u};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, estr,
+  int lower[2] = {-d->pad_w, -d->pad_h};
+  int upper[2] = {d->pad_w - (d->taps_w - 1), d->pad_h - (d->taps_h - 1)};
+  cuuint32_t estr[4] = {1u, (cuuint32_t)d->stride, (cuuint32_t)d->stride, 1u};
+  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, lower, upper, 64u,
+                   (cuuint32_t)kBlockM, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS;
+}
+
+// A operand of a 1x1 / stride-1 launch: 2-D [pixels, C] map, row stride ld elements.
+bool make_rows_map(CUtensorMap* m, const void* ptr, int c, int ld, long long pixels) {
+  EncodeTiledFn enc = get_encode();
+  if (!enc) return false;
+  cuuint64_t dims[2] = {(cuuint64_t)c, (cuuint64_t)pixels};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
+  cuuint32_t box[2] = {64u, (cuuint32_t)kBlockM};
+  cuuint32_t estr[2] = {1u, 1u};
+  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS;
+}
+
+bool make_act_map(CUtensorMap* m, const void* ptr, int c, int ld, const mdb_gemm_desc* d, bool im2col) {
+  return im2col ? make_im2col_map(m, ptr, c, ld, d)
+                : make_rows_map(m, ptr, c, ld, (long long)d->n_img * d->h_out * d->w_out);
 }
 
 bool make_w_map(CUtensorMap* m, const void* ptr, int n_out, int k, int block_n) {
@@ -45,7 +67,7 @@ bool make_w_map(CUtensorMap* m, const void* ptr, int n_out, int k, int block_n) 
 }
 
 struct Plan {
-  int bn, bh, bw, tiles_n, tiles_h, tiles_w;
+  int m_tiles;  // ceil(pixels / 128): tiles of consecutive output pixels
   int ctas, m_groups;  // CTAs per cluster (1, or 2 = CTA pairs) and M-tile groups walked by one cluster
   int block_n, n_tiles, splits, kb_per_split, kb_total;
 };
@@ -58,32 +80,6 @@ int num_sms() {
     if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
   }
   return sms;
-}
-
-// Choose the (bn, bh, bw) output-pixel box of one 128-row M tile: maximise the fraction of useful rows.
-void choose_box(int n_img, int h, int w, Plan* pl) {
-  if (h * w <= 128) {
-    int bn = 128 / (h * w);
-    if (bn > n_img) bn = n_img;
-    if (bn < 1) bn = 1;
-    pl->bn = bn, pl->bh = h, pl->bw = w;
-  } else {
-    double best = -1.0;
-    int bbh = 1, bbw = 1;
-    const int wmax = w < 128 ? w : 128;
-    for (int bw = 1; bw <= wmax; ++bw) {
-      int bh = 128 / bw;
-      if (bh > h) bh = h;
-      if (bh < 1) continue;
-      const long long tiles = (long long)((h + bh - 1) / bh) * ((w + bw - 1) / bw);
-      const double eff = (double)h * w / (double)(tiles * 128);
-      if (eff > best + 1e-9 || (eff > best - 1e-9 && bw > bbw)) best = eff, bbh = bh, bbw = bw;
-    }
-    pl->bn = 1, pl->bh = bbh, pl->bw = bbw;
-  }
-  pl->tiles_n = (n_img + pl->bn - 1) / pl->bn;
-  pl->tiles_h = (h + pl->bh - 1) / pl->bh;
-  pl->tiles_w = (w + pl->bw - 1) / pl->bw;
 }
 
 int validate(const mdb_gemm_desc* d) {
@@ -111,8 +107,8 @@ int validate(const mdb_gemm_desc* d) {
 
 // Tile width / split-K plan for `ctas` CTAs per cluster.
 void plan_for(const mdb_gemm_desc* d, int ctas, bool allow_split, Plan* pl) {
-  choose_box(d->n_img, d->h_out, d->w_out, pl);
-  const int m_tiles = pl->tiles_n * pl->tiles_h * pl->tiles_w;
+  const int m_tiles = (int)(((long long)d->n_img * d->h_out * d->w_out + kBlockM - 1) / kBlockM);
+  pl->m_tiles = m_tiles;
   pl->ctas = ctas;
   pl->m_groups = (m_tiles + ctas - 1) / ctas;
   pl->kb_total = d->taps_h * d->taps_w * ((d->c0 + d->c1) / 64);
@@ -226,6 +222,20 @@ extern "C" int mdb_gemm_conv_stats_parts(const mdb_gemm_desc* d) {
   return pl.n_tiles;  // one (sum, sum sq) slot per row and N tile
 }
 
+extern "C" int mdb_gemm_conv_plan(const mdb_gemm_desc* d, int* plan) {
+  if (validate(d) != MDB_OK) return MDB_ERR_INVALID;
+  Plan pl;
+  make_plan(d, &pl);
+  const long long walk = (long long)pl.m_groups * pl.n_tiles * pl.splits;
+  const int clusters = num_sms() / pl.ctas;
+  plan[0] = pl.block_n;
+  plan[1] = pl.m_tiles;
+  plan[2] = pl.n_tiles;
+  plan[3] = pl.splits;
+  plan[4] = (int)((walk + clusters - 1) / clusters);
+  return MDB_OK;
+}
+
 extern "C" int mdb_gemm_conv(const mdb_gemm_desc* d, void* stream) {
   int rc = validate(d);
   if (rc != MDB_OK) return rc;
@@ -236,13 +246,17 @@ extern "C" int mdb_gemm_conv(const mdb_gemm_desc* d, void* stream) {
   if (d->epi_mode == 1 && pl.block_n != 256) return set_error(MDB_ERR_UNSUPPORTED, "GEGLU needs block_n 256");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 
+  // output pixel p reads input pixel p unless the filter, stride, padding or output size say otherwise
+  const bool im2col = d->taps_h != 1 || d->taps_w != 1 || d->stride != 1 || d->pad_h || d->pad_w ||
+                      d->h_in != d->h_out || d->w_in != d->w_out;
   CUtensorMap tA0, tA1, tB;
-  if (!make_act_map(&tA0, d->a0, d->c0, d->lda0, d->n_img, d->h_in, d->w_in, pl.bn, pl.bh, pl.bw, d->stride))
-    return set_error(MDB_ERR_CUDA, "cuTensorMapEncodeTiled(A0) failed (c=%d ld=%d n=%d h=%d w=%d box=%dx%dx%d s=%d)",
-                     d->c0, d->lda0, d->n_img, d->h_in, d->w_in, pl.bn, pl.bh, pl.bw, d->stride);
+  if (!make_act_map(&tA0, d->a0, d->c0, d->lda0, d, im2col))
+    return set_error(MDB_ERR_CUDA, "cuTensorMapEncode%s(A0) failed (c=%d ld=%d n=%d h=%d w=%d taps=%dx%d pad=%dx%d s=%d)",
+                     im2col ? "Im2col" : "Tiled", d->c0, d->lda0, d->n_img, d->h_in, d->w_in, d->taps_h, d->taps_w,
+                     d->pad_h, d->pad_w, d->stride);
   if (d->c1 > 0) {
-    if (!make_act_map(&tA1, d->a1, d->c1, d->lda1, d->n_img, d->h_in, d->w_in, pl.bn, pl.bh, pl.bw, d->stride))
-      return set_error(MDB_ERR_CUDA, "cuTensorMapEncodeTiled(A1) failed");
+    if (!make_act_map(&tA1, d->a1, d->c1, d->lda1, d, im2col))
+      return set_error(MDB_ERR_CUDA, "cuTensorMapEncode%s(A1) failed", im2col ? "Im2col" : "Tiled");
   } else {
     tA1 = tA0;
   }
@@ -255,8 +269,8 @@ extern "C" int mdb_gemm_conv(const mdb_gemm_desc* d, void* stream) {
   gp.n_img = d->n_img, gp.h_out = d->h_out, gp.w_out = d->w_out, gp.n_out = d->n_out;
   gp.taps_h = d->taps_h, gp.taps_w = d->taps_w, gp.stride = d->stride, gp.pad_h = d->pad_h, gp.pad_w = d->pad_w;
   gp.cblocks0 = d->c0 / 64, gp.cblocks1 = d->c1 / 64;
-  gp.bn = pl.bn, gp.bh = pl.bh, gp.bw = pl.bw, gp.tiles_h = pl.tiles_h, gp.tiles_w = pl.tiles_w;
-  gp.m_tiles = pl.tiles_n * pl.tiles_h * pl.tiles_w, gp.n_tiles = pl.n_tiles, gp.splits = pl.splits;
+  gp.im2col = im2col;
+  gp.m_tiles = pl.m_tiles, gp.n_tiles = pl.n_tiles, gp.splits = pl.splits;
   gp.m_groups = pl.m_groups;
   gp.kb_per_split = pl.kb_per_split;
   gp.epi_mode = pl.splits > 1 ? EPI_PARTIAL_F32 : d->epi_mode;

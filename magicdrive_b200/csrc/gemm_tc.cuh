@@ -4,10 +4,12 @@
 //
 //   D[pixel, n] = sum_{tap, c}  A[pixel shifted by tap, c] * W[n, tap*C + c]      (+ epilogue)
 //
-// * A is an NHWC bf16 activation tensor addressed through a 4-D TMA tensor map (C, W, H, N innermost-first).
-//   One CTA owns a 128-row M tile that is a (bn x bh x bw) box of output pixels; each filter tap is the same
-//   box shifted by (r - pad_h, s - pad_w) and TMA zero-fills the out-of-bounds halo, so there is no im2col.
-//   Stride-2 convolutions use the tensor map's element strides.  A plain GEMM is the 1x1 / 1-image case.
+// * A is an NHWC bf16 activation tensor.  M tile mt is the 128 consecutive output pixels [128 mt, 128 mt + 128) of the
+//   flattened (image, row, column) order, whatever the image and row boundaries, so only the last tile has idle rows.
+//   - Convolutions (taps > 1, stride or padding): a 4-D (C, W, H, N) TMA map in im2col mode.  Each filter tap loads the
+//     tile's 128 pixels shifted by (s, r); the TMA walks across row and image ends, zero-fills the halo and the pixels
+//     past the last image, and steps by the stride through the map's element strides.  No im2col buffer exists.
+//   - 1x1 / stride-1 launches (plain GEMMs): a 2-D [pixels, C] tiled map with row stride lda.
 //   Two A sources are supported (the K loop runs over source 0's channels then source 1's): this is how
 //   channel-concatenated inputs (UNet skip connections) are consumed without materialising the concat.
 // * W is a bf16 [N, K] (K-major) matrix behind a 2-D tensor map, K ordered (tap, channel).
@@ -27,10 +29,8 @@ struct GemmParams {
   // filter
   int taps_h, taps_w, stride, pad_h, pad_w;
   int cblocks0, cblocks1;  // 64-channel blocks of A source 0 / 1
-  // M-tile box
-  int bn, bh, bw;
-  int tiles_h, tiles_w;  // tiles per image column/row direction
-  int m_tiles, n_tiles, splits;  // tiles = m_tiles * n_tiles * splits (m fastest)
+  int im2col;              // A maps: 1 = 4-D im2col (convolutions), 0 = 2-D [pixels, C] (1x1)
+  int m_tiles, n_tiles, splits;  // tiles = m_tiles * n_tiles * splits (m fastest); m_tiles = ceil(pixels / 128)
   int m_groups;                  // ceil(m_tiles / CTAS): M tiles are walked in groups of one per CTA of a cluster
   int kb_per_split;
   // epilogue

@@ -1,10 +1,10 @@
 // Persistent warp-specialised wgmma GEMM / implicit-GEMM convolution for sm_90a (operand scheme: gemm_tc.cuh).
 //
 // One CTA per SM loops over output tiles (m fastest, so concurrently running CTAs share the same weight tile in L2).
-//   warp 8:     TMA producer (one lane): A box + B tile per 64-wide K block into a ring of shared-memory stages; the ring
+//   warp 8:     TMA producer (one lane): A tile + B tile per 64-wide K block into a ring of shared-memory stages; the ring
 //               keeps flowing across tile boundaries, so the loads of tile i+1 overlap the epilogue of tile i.
 //   CTAS = 2:   CTA pairs.  The two CTAs of a cluster compute consecutive M tiles against the same weight tile; each loads
-//               its own A box and HALF of the B tile, multicast into both CTAs' shared memory, which halves the L2 -> SM
+//               its own A tile and HALF of the B tile, multicast into both CTAs' shared memory, which halves the L2 -> SM
 //               weight traffic.  A stage is refilled only once the consumers of BOTH CTAs have released it (every
 //               consumer warp arrives on the empty barrier of both CTAs).
 //   warps 0..7: two consumer warpgroups, rows [0, 64) and [64, 128) of the 128-row M tile: wgmma m64 x BLOCK_N x k16 with
@@ -81,7 +81,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
   if (warp == Cfg::kConsumerWarps) {
     // =========================== TMA producer ===========================
     if (lane == 0) {
-      const uint32_t tx_bytes = static_cast<uint32_t>(p.bn * p.bh * p.bw) * (kBlockK * 2) + Cfg::kBBytes;
+      const uint32_t tx_bytes = kABytes + Cfg::kBBytes;  // out-of-bounds rows are zero-filled and still counted
+      const int hw_out = p.h_out * p.w_out;
       int stage = 0;
       uint32_t phase = 0;
       for (int t = first_tile; t < total_tiles; t += tile_step) {
@@ -89,10 +90,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
         const int rest = t / p.m_groups;
         const int nt = rest % p.n_tiles;
         const int z = rest / p.n_tiles;
-        const int tw = mt % p.tiles_w;
-        const int th = (mt / p.tiles_w) % p.tiles_h;
-        const int tn = mt / (p.tiles_w * p.tiles_h);
-        const int img0 = tn * p.bn, h0 = th * p.bh, w0 = tw * p.bw;
+        // im2col start: input position of the tile's first output pixel (the top-left filter tap)
+        const int pix0 = mt * kBlockM;
+        const int img0 = pix0 / hw_out;
+        const int oh0 = (pix0 - img0 * hw_out) / p.w_out;
+        const int ow0 = pix0 - img0 * hw_out - oh0 * p.w_out;
+        const int wc = ow0 * p.stride - p.pad_w, hc = oh0 * p.stride - p.pad_h;
         const int n0 = nt * BLOCK_N;
         const int kb_begin = z * p.kb_per_split;
         const int kb_end = min(kb_total, kb_begin + p.kb_per_split);
@@ -102,12 +105,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
           const int cb = kb - tap * cb_total;
           const int r = tap / p.taps_w, s = tap - r * p.taps_w;
           mbar_arrive_expect_tx(&full_bar[stage], tx_bytes);
-          const int wc = w0 * p.stride + s - p.pad_w;
-          const int hc = h0 * p.stride + r - p.pad_h;
-          if (cb < p.cblocks0)
-            tma_load_4d(&tmA0, &full_bar[stage], smA + stage * kABytes, cb * kBlockK, wc, hc, img0);
+          const CUtensorMap* tmA = cb < p.cblocks0 ? &tmA0 : &tmA1;
+          const int c = (cb < p.cblocks0 ? cb : cb - p.cblocks0) * kBlockK;
+          if (p.im2col)
+            tma_load_im2col_4d(tmA, &full_bar[stage], smA + stage * kABytes, c, wc, hc, img0, static_cast<uint16_t>(s),
+                               static_cast<uint16_t>(r));
           else
-            tma_load_4d(&tmA1, &full_bar[stage], smA + stage * kABytes, (cb - p.cblocks0) * kBlockK, wc, hc, img0);
+            tma_load_2d(tmA, &full_bar[stage], smA + stage * kABytes, c, pix0);
           if constexpr (PAIR)
             tma_load_2d_multicast(&tmB, &full_bar[stage], smB + stage * Cfg::kBBytes + rank * Cfg::kBPartBytes, kb * kBlockK,
                                   n0 + rank * Cfg::kBRows, 0x3);
@@ -125,16 +129,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
   const int wg = warp >> 2;
   const int q = lane & 3;
   const int row0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // this thread's accumulator rows: row0 and row0 + 8
-  const int box_hw = p.bh * p.bw;
-  int li[2], lh[2], lw[2];
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int row = row0 + 8 * h;
-    li[h] = row / box_hw;
-    const int rem = row - li[h] * box_hw;
-    lh[h] = rem / p.bw;
-    lw[h] = rem - lh[h] * p.bw;
-  }
+  const int hw_out = p.h_out * p.w_out;
   const long long pixels_total = static_cast<long long>(p.n_img) * p.h_out * p.w_out;
   const float scale = p.out_scale;
   int stage = 0;
@@ -151,9 +146,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
     const int rest = t / p.m_groups;
     const int nt = rest % p.n_tiles;
     const int z = rest / p.n_tiles;
-    const int tw = mt % p.tiles_w;
-    const int th = (mt / p.tiles_w) % p.tiles_h;
-    const int tn = mt / (p.tiles_w * p.tiles_h);
     const int n0 = nt * BLOCK_N;
     const int kb_begin = z * p.kb_per_split;
     const int nkb = min(kb_total, kb_begin + p.kb_per_split) - kb_begin;
@@ -188,10 +180,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
     bool ok[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      img[h] = tn * p.bn + li[h];
-      const int oh = th * p.bh + lh[h], ow = tw * p.bw + lw[h];
-      ok[h] = (li[h] < p.bn) && (img[h] < p.n_img) && (oh < p.h_out) && (ow < p.w_out);
-      pix[h] = (static_cast<long long>(img[h]) * p.h_out + oh) * p.w_out + ow;
+      const int px = mt * kBlockM + row0 + 8 * h;
+      img[h] = px / hw_out;
+      pix[h] = px;
+      ok[h] = pix[h] < pixels_total;
     }
     if (p.epi_mode == EPI_PARTIAL_F32) {
 #pragma unroll

@@ -179,9 +179,13 @@ def gemm_conv(a0: torch.Tensor, w: torch.Tensor, *, n_img: int, h_in: int, w_in:
         d.stats_out = stats.data.data_ptr()
     e0 = _prof_begin()
     check(L.mdb_gemm_conv(C.byref(d), _stream()), "mdb_gemm_conv")
-    _prof_end("gemm_conv", 2.0 * pixels * n_out * taps * taps * (c0 + c1), e0,
-              f"M={pixels} N={n_out} K={taps * taps * (c0 + c1)} img={n_img}x{h_out}x{w_out} taps={taps} s={stride} "
-              f"geglu={int(geglu)} res={int(residual is not None)}")
+    if e0 is not None:
+        plan = (C.c_int * 5)()
+        check(L.mdb_gemm_conv_plan(C.byref(d), plan), "mdb_gemm_conv_plan")
+        _prof_end("gemm_conv", 2.0 * pixels * n_out * taps * taps * (c0 + c1), e0,
+                  f"M={pixels} N={n_out} K={taps * taps * (c0 + c1)} img={n_img}x{h_out}x{w_out} taps={taps} s={stride} "
+                  f"geglu={int(geglu)} res={int(residual is not None)} | BN={plan[0]} tiles={plan[1]}x{plan[2]}x{plan[3]} "
+                  f"waves={plan[4]}")
     _launches += L.mdb_gemm_conv_launches(C.byref(d))
     return (out, stats) if emit_stats else out
 
