@@ -37,12 +37,22 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
   return u;
 }
 
-// ---- GroupNorm pass 1: per (image, group) sum / sum-of-squares.  blockDim = vpp * R, thread = (pixel lane r, channel vector cv)
+// Shift of group g of an image for the two-kernel statistics: the image's first pixel, first channel of the group.  Sums of
+// (x - shift) keep E[d^2] - E[d]^2 well conditioned: a sample of the group lies within a few standard deviations of its mean,
+// whereas the plain E[x^2] - mean^2 in fp32 is off by several percent once |mean| is a few hundred standard deviations.
+__device__ __forceinline__ float gn_shift(const __nv_bfloat16* __restrict__ x0, int c0, int ld0,
+                                          const __nv_bfloat16* __restrict__ x1, int ld1, long long pix, int c) {
+  return __bfloat162float(c < c0 ? x0[pix * ld0 + c] : x1[pix * ld1 + (c - c0)]);
+}
+
+// ---- GroupNorm pass 1: per (image, group) sum / sum-of-squares of x - shift.  blockDim = vpp * R, thread = (pixel lane r,
+// channel vector cv)
 __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x0, int c0, int ld0,
                                 const __nv_bfloat16* __restrict__ x1, int c1, int ld1, int hw, int groups, int vpp,
                                 int R, int pix_per_cta, float* __restrict__ stats) {
   extern __shared__ float sm[];  // [2][ctot]
   const int ctot = c0 + c1;
+  const int cpg = ctot / groups;
   const int img = blockIdx.y;
   const int p_begin = blockIdx.x * pix_per_cta;
   const int p_end = min(hw, p_begin + pix_per_cta);
@@ -56,15 +66,21 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x0, int c0, in
     int ld, coff;
     if (ch < c0) base = x0, ld = ld0, coff = ch;
     else base = x1, ld = ld1, coff = ch - c0;
-    float s[8], ss[8];
+    float s[8], ss[8], k[8];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) s[i] = 0.f, ss[i] = 0.f;
+    for (int i = 0; i < 8; ++i) {
+      s[i] = 0.f, ss[i] = 0.f;
+      k[i] = gn_shift(x0, c0, ld0, x1, ld1, static_cast<long long>(img) * hw, (ch + i) / cpg * cpg);
+    }
     for (int p = p_begin + r; p < p_end; p += R) {
       const uint4 u = __ldg(reinterpret_cast<const uint4*>(base + (static_cast<long long>(img) * hw + p) * ld + coff));
       float f[8];
       unpack8(u, f);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) s[i] += f[i], ss[i] += f[i] * f[i];
+      for (int i = 0; i < 8; ++i) {
+        const float d = f[i] - k[i];
+        s[i] += d, ss[i] += d * d;
+      }
     }
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -73,7 +89,6 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x0, int c0, in
     }
   }
   __syncthreads();
-  const int cpg = ctot / groups;
   for (int g = threadIdx.x; g < groups; g += blockDim.x) {
     float a = 0.f, b = 0.f;
     for (int c = g * cpg; c < (g + 1) * cpg; ++c) a += sm[c], b += sm[ctot + c];
@@ -82,7 +97,8 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x0, int c0, in
   }
 }
 
-// ---- GroupNorm pass 2: y = (x - mean) * rstd * gamma + beta, optional SiLU, bf16 out.
+// ---- GroupNorm pass 2: mean = shift + E[x - shift], var = E[(x - shift)^2] - E[x - shift]^2;
+// y = (x - mean) * rstd * gamma + beta, optional SiLU, bf16 out.
 __global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x0, int c0, int ld0,
                                 const __nv_bfloat16* __restrict__ x1, int c1, int ld1, int hw, int groups, float eps,
                                 const float* __restrict__ gamma, const float* __restrict__ beta, int silu,
@@ -95,9 +111,10 @@ __global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x0, int c0, in
   const float inv_cnt = 1.0f / (static_cast<float>(cpg) * static_cast<float>(hw));
   for (int c = threadIdx.x; c < ctot; c += blockDim.x) {
     const int g = c / cpg;
-    const float mean = stats[(img * groups + g) * 2] * inv_cnt;
-    float var = stats[(img * groups + g) * 2 + 1] * inv_cnt - mean * mean;
+    const float dmean = stats[(img * groups + g) * 2] * inv_cnt;  // mean of x - shift
+    float var = stats[(img * groups + g) * 2 + 1] * inv_cnt - dmean * dmean;
     var = fmaxf(var, 0.f);
+    const float mean = gn_shift(x0, c0, ld0, x1, ld1, static_cast<long long>(img) * hw, g * cpg) + dmean;
     const float rstd = rsqrtf(var + eps);
     const float a = rstd * gamma[c];
     sm[c] = a;
