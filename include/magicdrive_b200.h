@@ -67,7 +67,9 @@ typedef struct {
   int ldo;
   int out_is_f32;
   float out_scale;
-  int epi_mode;         /* 0 linear, 1 GEGLU */
+  int epi_mode;         /* 0 linear, 1 GEGLU, 2 quick-GELU: out = y * sigmoid(1.702 y) on y = the linear epilogue's value
+                         * (CLIP MLP fc1, transformers models/clip/modeling_clip.py CLIPMLP); never split-K, no residual,
+                         * rowbias, stats_out or fp32 output */
   void* workspace;      /* split-K scratch (may be NULL => no split-K) */
   size_t workspace_bytes;
   int force_block_n;    /* 0 = auto; test hook */
@@ -141,6 +143,21 @@ int mdb_attention(const void* q, int ldq, const void* k, int ldk, const void* v,
 int mdb_attention_multi(const void* q, int ldq, int n_src, const void* const* k, const int* ldk, const void* const* v,
                         const int* ldv, const int* b_kv, void* out, int ldo, int b, int heads, int lq, int lk, int d,
                         const int* kv_index, int n_sets, float scale, void* stream);
+
+/* Causal self-attention of the CLIP text encoder (transformers models/clip/modeling_clip.py CLIPAttention.forward with the
+ * causal_attention_mask of CLIPTextTransformer.forward): as mdb_attention with one set, b_kv == b and no kv_index, and key j
+ * visible to query i iff j <= i.  Requires lq == lk (MDB_ERR_INVALID otherwise).  Key tiles wholly above a query tile's
+ * diagonal are neither loaded nor computed.  Same head dims and MDB_ATTN_KERNEL variants as mdb_attention. */
+int mdb_attention_causal(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, void* out, int ldo, int b,
+                         int heads, int lq, int lk, int d, float scale, void* stream);
+
+/* CLIP token + position embedding (modeling_clip.py CLIPTextEmbeddings.forward): for row r = s * len + p of n_seq sequences
+ * of len tokens, out[r, :dim] = bf16(tok[ids[r]] + pos[p]) and stats_out[r] = (sum, sum of squares) of that bf16 row: the
+ * fp32 [rows, 1, 2] row statistics a GEMM with a folded LayerNorm reads (ln_parts = 1).  ids: device int32, or int64 if
+ * ids_are_i64; an id outside [0, vocab) gives a NaN row (and NaN statistics) and is never used as an address.
+ * tok_table_bf16 [vocab, dim], pos_table_bf16 [>= len, dim]; dim and ldo multiples of 8. */
+int mdb_clip_embed(const void* ids, int ids_are_i64, int n_seq, int len, const void* tok_table_bf16, int vocab,
+                   const void* pos_table_bf16, int dim, void* out_bf16, int ldo, float* stats_out, void* stream);
 
 /* out = a + b (bf16), n elements (unet_2d_condition_multiview.py:464-473, 487-488). */
 int mdb_add(const void* a, const void* b, void* out, long long n, void* stream);

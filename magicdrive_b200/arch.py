@@ -382,6 +382,43 @@ def vae_decoder_param_shapes(cfg: VaeConfig) -> "OrderedDict[str, tuple]":
     return sh
 
 
+# ------------------------------------------------------------------------------------------ CLIP text encoder
+@dataclass
+class ClipTextConfig:
+    """CLIPTextConfig of SD-1.5's text_encoder/config.json (CLIP ViT-L/14 text tower): pre-LN transformer with causal
+    self-attention and a quick_gelu MLP (transformers models/clip/configuration_clip.py, modeling_clip.py)."""
+    vocab_size: int = 49408
+    hidden_size: int = 768
+    intermediate_size: int = 3072
+    num_hidden_layers: int = 12
+    num_attention_heads: int = 12
+    max_position_embeddings: int = 77
+    hidden_act: str = "quick_gelu"
+    layer_norm_eps: float = 1e-5
+    bos_token_id: int = 0
+    eos_token_id: int = 2
+    pad_token_id: int = 1
+    projection_dim: int = 768
+
+
+def clip_text_param_shapes(cfg: ClipTextConfig) -> "OrderedDict[str, tuple]":
+    """CLIPTextModel.state_dict() keys (196 at SD-1.5 size): text_model.embeddings.*, .encoder.layers.N.*, .final_layer_norm."""
+    sh: "OrderedDict[str, tuple]" = OrderedDict()
+    c, t = cfg.hidden_size, "text_model"
+    sh[t + ".embeddings.token_embedding.weight"] = (cfg.vocab_size, c)
+    sh[t + ".embeddings.position_embedding.weight"] = (cfg.max_position_embeddings, c)
+    for i in range(cfg.num_hidden_layers):
+        p = f"{t}.encoder.layers.{i}"
+        for n in ("k_proj", "v_proj", "q_proj", "out_proj"):
+            _lin(sh, f"{p}.self_attn.{n}", c, c)
+        _norm(sh, p + ".layer_norm1", c)
+        _lin(sh, p + ".mlp.fc1", cfg.intermediate_size, c)
+        _lin(sh, p + ".mlp.fc2", c, cfg.intermediate_size)
+        _norm(sh, p + ".layer_norm2", c)
+    _norm(sh, t + ".final_layer_norm", c)
+    return sh
+
+
 BUFFER_KEYS = {"bbox_embedder._class_tokens"}
 
 

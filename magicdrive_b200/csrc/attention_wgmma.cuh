@@ -11,6 +11,9 @@
 //   (each rounded to bf16 first, like the reference's per-branch outputs).
 //   Multi-Q mode (p.q_step > 0): the CTA walks the query tiles blockIdx.x, blockIdx.x + q_step, ... of its (batch, head);
 //   with a single K/V tile (lk <= BN, one set: the text / camera / box cross-attention) that tile is loaded once.
+//   CAUSAL (self-attention with lq == lk, one set): key j is visible to query i iff j <= i.  A query tile walks only the key
+//   tiles up to the one holding its last row's diagonal (ascending, so tile 0, which holds key 0, always comes first), and
+//   producer and consumers derive that count from the same q0.
 #pragma once
 #include "ptx.cuh"
 #include "wgmma.cuh"
@@ -58,7 +61,7 @@ struct AttnCfg {
   static_assert(STAGES >= 1 && kSmemBytes <= 232448, "shared memory");
 };
 
-template <int D, int BN_>
+template <int D, int BN_, bool CAUSAL = false>
 __global__ void __launch_bounds__(AttnCfg<D, BN_>::kThreads, 1)
 attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ AttnKvMaps kvm, const AttnParams p) {
   using Cfg = AttnCfg<D, BN_>;
@@ -83,6 +86,8 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
   const int n_own = (nq - static_cast<int>(blockIdx.x) + q_step - 1) / q_step;  // query tiles of this CTA
   const bool kv_resident = ntiles == 1 && p.n_sets == 1 && n_own > 1;
   auto q0_of = [&](int o) { return (static_cast<int>(blockIdx.x) + o * q_step) * ATT_BM; };
+  // key tiles a query tile starting at q0 reads: causal tiles stop at the one holding key min(q0 + ATT_BM, lq) - 1
+  auto tiles_of = [&](int q0) { return CAUSAL ? min(ntiles, (min(q0 + ATT_BM, p.lq) - 1) / BN + 1) : ntiles; };
 
   if (warp == Cfg::kConsumerWarps && lane == 0) {
     prefetch_tmap(&tmQ);
@@ -118,7 +123,8 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
           const int kvb = kve & 0xffffff;
           const CUtensorMap* km = &kvm.k[kve >> 24];
           const CUtensorMap* vm = &kvm.v[kve >> 24];
-          for (int j = 0; j < ntiles; ++j) {
+          const int nt = tiles_of(q0_of(o));
+          for (int j = 0; j < nt; ++j) {
             mbar_wait(&kv_empty[stage], phase ^ 1);
             mbar_arrive_expect_tx(&kv_full[stage], 2 * KD * TILE_KV);
 #pragma unroll
@@ -152,7 +158,8 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
 #pragma unroll
       for (int i = 0; i < Cfg::OACC; ++i) oacc[i] = 0.f;
       float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
-      for (int j = 0; j < ntiles; ++j) {
+      const int nt = tiles_of(q0);
+      for (int j = 0; j < nt; ++j) {
         const int st = kv_resident ? 0 : stage;
         mbar_wait(&kv_full[st], kv_resident ? 0u : phase);
         // ---- S = Q K^T
@@ -176,6 +183,18 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
             for (int e = 0; e < 2; ++e)
               if (kbase + 8 * g + 2 * q + e >= p.lk) s[4 * g + e] = s[4 * g + 2 + e] = -INFINITY;
         }
+        // ---- causal: keys after the query row take no weight (only tiles that reach past the tile's first row)
+        if constexpr (CAUSAL) {
+          if (kbase + BN - 1 > q0 + rloc) {
+#pragma unroll
+            for (int g = 0; g < BN / 8; ++g)
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int e = 0; e < 2; ++e)
+                  if (kbase + 8 * g + 2 * q + e > q0 + rloc + 8 * h) s[4 * g + 2 * h + e] = -INFINITY;
+          }
+        }
         // ---- online softmax (row max over the quad that shares a row)
         float corr[2];
 #pragma unroll
@@ -185,7 +204,8 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
           for (int g = 0; g < BN / 8; ++g) mx = fmaxf(mx, fmaxf(s[4 * g + 2 * h], s[4 * g + 2 * h + 1]));
           mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
           mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-          const float m_new = fmaxf(m[h], mx * sc);  // sc > 0; finite: key kbase is always valid
+          // sc > 0; finite: key kbase is always valid (causal: key 0 of tile 0, walked first, is visible to every row)
+          const float m_new = fmaxf(m[h], mx * sc);
           corr[h] = exp2f(m[h] - m_new);
           m[h] = m_new;
         }

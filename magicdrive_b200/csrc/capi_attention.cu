@@ -6,6 +6,7 @@
 // BasicMultiviewTransformerBlock (magicdrive/networks/blocks.py:112-121, 213-217).  K/V may be spread over up to three
 // buffers (mdb_attention_multi): in view-sharded runs the neighbour views' K/V are read in place from the ring-neighbour
 // GPUs' buffers through NVLink peer memory (the tensor maps simply point at peer-mapped addresses).
+// mdb_attention_causal is the CLIP text encoder's masked self-attention (one set, one source, lq == lk).
 // Kernel: attention_wgmma.cuh.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -77,13 +78,13 @@ int multi_q_step(int b, int heads, int lq, int lk, int n_sets, int bn) {
   return static_cast<int>(gx);
 }
 
-template <int D, int BN_>
+template <int D, int BN_, bool CAUSAL>
 int launch_attention(const void* q, int ldq, const KvSources& src, void* out, int ldo, int b, int heads, int lq, int lk,
                      const int* kv_index, int n_sets, float scale, cudaStream_t st) {
   using Cfg = mdb::AttnCfg<D, BN_>;
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(mdb::attention_wgmma_kernel<D, BN_>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(mdb::attention_wgmma_kernel<D, BN_, CAUSAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e != cudaSuccess) return mdb::set_error(MDB_ERR_CUDA, "attention_wgmma_kernel smem attr: %s", cudaGetErrorString(e));
     attr = true;
   }
@@ -97,36 +98,37 @@ int launch_attention(const void* q, int ldq, const KvSources& src, void* out, in
   p.scale_log2 = scale * 1.4426950408889634f;
   p.q_step = multi_q_step(b, heads, lq, lk, n_sets, Cfg::BN);
   dim3 grid(p.q_step > 0 ? p.q_step : (lq + mdb::ATT_BM - 1) / mdb::ATT_BM, heads, b);
-  cudaError_t le = mdb::launch_pdl(mdb::attention_wgmma_kernel<D, BN_>, grid, dim3(Cfg::kThreads), Cfg::kSmemBytes, st, tq, kvm, p);
+  cudaError_t le = mdb::launch_pdl(mdb::attention_wgmma_kernel<D, BN_, CAUSAL>, grid, dim3(Cfg::kThreads), Cfg::kSmemBytes, st, tq, kvm, p);
   if (le != cudaSuccess) return mdb::set_error(MDB_ERR_CUDA, "attention_wgmma_kernel launch: %s", cudaGetErrorString(le));
   cudaError_t e2 = cudaGetLastError();
   if (e2 != cudaSuccess) return mdb::set_error(MDB_ERR_CUDA, "attention_wgmma_kernel: %s", cudaGetErrorString(e2));
   return MDB_OK;
 }
 
-template <int BN_>
+template <int BN_, bool CAUSAL>
 int attention_dispatch_bn(const void* q, int ldq, const KvSources& src, void* out, int ldo, int b, int heads, int lq, int lk, int d,
                           const int* kv_index, int n_sets, float scale, cudaStream_t st) {
   switch (d) {
-    case 32: return launch_attention<32, BN_>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
-    case 40: return launch_attention<40, BN_>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
-    case 64: return launch_attention<64, BN_>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
-    case 80: return launch_attention<80, BN_>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
-    case 160: return launch_attention<160, BN_>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
+    case 32: return launch_attention<32, BN_, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
+    case 40: return launch_attention<40, BN_, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
+    case 64: return launch_attention<64, BN_, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
+    case 80: return launch_attention<80, BN_, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
+    case 160: return launch_attention<160, BN_, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
     default: return mdb::set_error(MDB_ERR_UNSUPPORTED, "mdb_attention: head dim %d not instantiated (32, 40, 64, 80, 160)", d);
   }
 }
 
 // Key-tile width (A/B switch, read per call): MDB_ATTN_KERNEL = tc2 (default: 128 keys for head dims <= 64, 64 above) |
 // tc2d (64-key tiles: smaller S fragment, deeper K/V ring) | tc (128-key tiles for every head dim).
+template <bool CAUSAL = false>
 int attention_dispatch(const void* q, int ldq, const KvSources& src, void* out, int ldo, int b, int heads, int lq, int lk, int d,
                        const int* kv_index, int n_sets, float scale, cudaStream_t st) {
   const char* e = getenv("MDB_ATTN_KERNEL");
-  if (e && !strcmp(e, "tc2d")) return attention_dispatch_bn<64>(q, ldq, src, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, scale, st);
-  if (e && !strcmp(e, "tc")) return attention_dispatch_bn<128>(q, ldq, src, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, scale, st);
+  if (e && !strcmp(e, "tc2d")) return attention_dispatch_bn<64, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, scale, st);
+  if (e && !strcmp(e, "tc")) return attention_dispatch_bn<128, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, scale, st);
   if (e && *e && strcmp(e, "tc2"))
     return mdb::set_error(MDB_ERR_INVALID, "mdb_attention: MDB_ATTN_KERNEL must be tc2, tc2d or tc (got %s)", e);
-  return attention_dispatch_bn<0>(q, ldq, src, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, scale, st);
+  return attention_dispatch_bn<0, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, scale, st);
 }
 
 }  // namespace
@@ -157,4 +159,18 @@ extern "C" int mdb_attention(const void* q, int ldq, const void* k, int ldk, con
                              int b_kv, int heads, int lq, int lk, int d, const int* kv_index, int n_sets, float scale,
                              void* stream) {
   return mdb_attention_multi(q, ldq, 1, &k, &ldk, &v, &ldv, &b_kv, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, scale, stream);
+}
+
+extern "C" int mdb_attention_causal(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, void* out, int ldo,
+                                    int b, int heads, int lq, int lk, int d, float scale, void* stream) {
+  using namespace mdb;
+  if (!q || !k || !v || !out) return set_error(MDB_ERR_INVALID, "mdb_attention_causal: null pointer");
+  if (lq != lk) return set_error(MDB_ERR_INVALID, "mdb_attention_causal: lq (%d) must equal lk (%d)", lq, lk);
+  if (scale <= 0.f) return set_error(MDB_ERR_INVALID, "mdb_attention_causal: scale must be positive");
+  if (lq <= 0 || b <= 0 || heads <= 0) return set_error(MDB_ERR_INVALID, "mdb_attention_causal: bad shape");
+  if (ldq % 8 || ldk % 8 || ldv % 8 || ldo % 8) return set_error(MDB_ERR_UNSUPPORTED, "mdb_attention_causal: strides must be multiples of 8");
+  KvSources src;
+  src.n = 1;
+  src.k[0] = k, src.v[0] = v, src.ldk[0] = ldk, src.ldv[0] = ldv, src.b_kv[0] = b;
+  return attention_dispatch<true>(q, ldq, src, out, ldo, b, heads, lq, lk, d, nullptr, 1, scale, static_cast<cudaStream_t>(stream));
 }

@@ -102,6 +102,10 @@ int validate(const mdb_gemm_desc* d) {
   if (d->epi_mode == 1 && (d->n_out % 256 || d->residual || d->rowbias || d->out_is_f32 || d->stats_out))
     return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: GEGLU epilogue needs n_out %% 256 == 0 and a plain bf16 output "
                                           "(no residual, per-image shift or row statistics)");
+  if (d->epi_mode == 2 && (d->residual || d->rowbias || d->out_is_f32 || d->stats_out))
+    return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: quick-GELU epilogue needs a plain bf16 output "
+                                          "(no residual, per-image shift or row statistics)");
+  if (d->epi_mode < 0 || d->epi_mode > 2) return set_error(MDB_ERR_INVALID, "mdb_gemm_conv: epi_mode must be 0, 1 or 2");
   return MDB_OK;
 }
 
@@ -273,7 +277,7 @@ extern "C" int mdb_gemm_conv(const mdb_gemm_desc* d, void* stream) {
   gp.m_tiles = pl.m_tiles, gp.n_tiles = pl.n_tiles, gp.splits = pl.splits;
   gp.m_groups = pl.m_groups;
   gp.kb_per_split = pl.kb_per_split;
-  gp.epi_mode = pl.splits > 1 ? EPI_PARTIAL_F32 : d->epi_mode;
+  gp.epi_mode = pl.splits > 1 ? EPI_PARTIAL_F32 : d->epi_mode == 2 ? EPI_QUICK_GELU : d->epi_mode;
   gp.out_is_f32 = d->out_is_f32;
   gp.bias = d->bias, gp.rowbias = d->rowbias, gp.rowbias_ld = d->rowbias_ld;
   gp.residual = static_cast<const __nv_bfloat16*>(d->residual), gp.ldr = d->ldr;

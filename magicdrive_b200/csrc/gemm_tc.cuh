@@ -20,7 +20,8 @@
 
 namespace mdb {
 
-enum EpiMode : int { EPI_LINEAR = 0, EPI_GEGLU = 1, EPI_PARTIAL_F32 = 2 };
+// EPI_QUICK_GELU is mdb_gemm_desc.epi_mode 2 (internal 2 is the split-K partial store)
+enum EpiMode : int { EPI_LINEAR = 0, EPI_GEGLU = 1, EPI_PARTIAL_F32 = 2, EPI_QUICK_GELU = 3 };
 
 struct GemmParams {
   // output pixel grid
@@ -74,6 +75,15 @@ __device__ __forceinline__ float gelu_erf(float x) {
   const float erf_abs = fmaf(-poly, e, 1.0f);
   const float hx = 0.5f * x;
   return fmaf(hx, copysignf(erf_abs, x), hx);
+}
+
+// CLIP's quick_gelu x * sigmoid(1.702 x) (transformers activations.py QuickGELUActivation).  For x << 0 the exponential
+// overflows to +inf and the result is -0, the limit.
+__device__ __forceinline__ float quick_gelu(float x) {
+  float e, r;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(-1.702f * 1.4426950408889634f * x));
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
+  return x * r;
 }
 
 // Deterministic split-K finalisation: sum the fp32 partials in split order, then the same linear epilogue.

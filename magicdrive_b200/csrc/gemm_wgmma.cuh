@@ -239,6 +239,24 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
       }
       continue;
     }
+    if (p.epi_mode == EPI_QUICK_GELU) {  // its own loop, so the linear epilogue below stays as it is: plain bf16 output
+#pragma unroll
+      for (int j = 0; j < BLOCK_N / 8; ++j) {
+        const int col = n0 + 8 * j + 2 * q;
+        if (col >= p.n_out) continue;
+        const float2 b = p.bias ? ldg_f2(p.bias + col) : make_float2(0.f, 0.f);
+        const float2 cs = has_ln ? ldg_f2(p.ln_colsum + col) : make_float2(0.f, 0.f);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!ok[h]) continue;
+          const float v0 = fmaf(rowA[h], acc[4 * j + 2 * h], fmaf(rowB[h], cs.x, b.x * scale));
+          const float v1 = fmaf(rowA[h], acc[4 * j + 2 * h + 1], fmaf(rowB[h], cs.y, b.y * scale));
+          *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.out) + pix[h] * p.ldo + col) =
+              pack_bf16(quick_gelu(v0), quick_gelu(v1));
+        }
+      }
+      continue;
+    }
     float st_s[2] = {0.f, 0.f}, st_ss[2] = {0.f, 0.f};
 #pragma unroll
     for (int j = 0; j < BLOCK_N / 8; ++j) {

@@ -689,3 +689,47 @@ class VaeDecoderEngine:
                             bias=bo, out_f32=True, out_scale=0.5 if to_unit_range else 1.0)
         img = img.reshape(x.n, x.h, x.w, self.COUT_PAD)[..., : cfg.out_channels]
         return img.clamp(0, 1) if to_unit_range else img
+
+
+class TextEncoderEngine:
+    """CLIPTextModel.forward (transformers models/clip/modeling_clip.py: CLIPTextTransformer.forward -> CLIPEncoderLayer)
+    on the same operators as the denoiser's transformer blocks: the residual stream X is bf16 [n*L, C]; every operator that
+    writes X also emits its row statistics, and layer_norm1 / layer_norm2 are folded into the QKV and fc1 GEMMs that read X
+    (no LayerNorm kernel inside a layer).  Attention is the causal fused kernel reading the QKV GEMM's output in place;
+    fc1 applies quick_gelu in its epilogue; final_layer_norm is one mdb_layernorm.  This replaces the reference's
+    `text_encoder(ids)` calls (pipeline_controlnet.py:365-369, 417-421; bbox_embedder.py:123-135)."""
+
+    def __init__(self, cfg: arch.ClipTextConfig, sd, device):
+        self.cfg, self.device = cfg, device
+        self.W = _Weights(sd, device)
+
+    def forward(self, ids: torch.Tensor):
+        """ids: int32 / int64 [n, L] on the device, L <= max_position_embeddings.  Returns (last_hidden_state bf16
+        [n, L, C], pooler_output bf16 [n, C]); the pooled row is the one at argmax(ids) (the SD-1.5 config's eos_token_id
+        == 2 rule of CLIPTextTransformer.forward)."""
+        cfg, W = self.cfg, self.W
+        n, L = ids.shape
+        C, heads, eps = cfg.hidden_size, cfg.num_attention_heads, cfg.layer_norm_eps
+        d = C // heads
+        t = "text_model"
+        if t + ".tok" not in W.t:
+            W.t[t + ".tok"] = _bf(W.raw(t + ".embeddings.token_embedding.weight"))
+            W.t[t + ".pos"] = _bf(W.raw(t + ".embeddings.position_embedding.weight"))
+        X, sx = ops.clip_embed(ids, W.t[t + ".tok"], W.t[t + ".pos"])
+        for i in range(cfg.num_hidden_layers):
+            p = f"{t}.encoder.layers.{i}"
+            a = p + ".self_attn"
+            wqkv, cqkv, sqkv = W.ln_lin(a + ".lnqkv", p + ".layer_norm1", [a + ".q_proj", a + ".k_proj", a + ".v_proj"])
+            qkv = ops.linear(X, wqkv, bias=cqkv, ln=sx, ln_colsum=sqkv, ln_eps=eps)
+            o = ops.attention_causal(qkv, qkv[:, C:], qkv[:, 2 * C:], b=n, heads=heads, l=L, d=d, ldq=3 * C, ldk=3 * C,
+                                     ldv=3 * C, scale=d ** -0.5)
+            wo, bo = W.lin(a + ".out_proj")
+            X, sx = ops.linear(o, wo, bias=bo, residual=X, emit_stats=True)
+            w1, c1, s1 = W.ln_lin(p + ".mlp.lnfc1", p + ".layer_norm2", [p + ".mlp.fc1"])
+            h = ops.linear(X, w1, bias=c1, ln=sx, ln_colsum=s1, ln_eps=eps, quick_gelu=True)
+            w2, b2 = W.lin(p + ".mlp.fc2")
+            X, sx = ops.linear(h, w2, bias=b2, residual=X, emit_stats=True)
+        g, b = W.norm(t + ".final_layer_norm")
+        out = ops.layernorm(X, g, b, eps).view(n, L, C)
+        pooled = out[torch.arange(n, device=out.device), ids.argmax(-1)]
+        return out, pooled

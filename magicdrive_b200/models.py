@@ -1,4 +1,4 @@
-"""Drop-in modules for the two networks of the hot path.
+"""Drop-in modules for the two networks of the hot path, and for the VAE decoder and CLIP text encoder around it.
 
 `UNet2DConditionModelMultiview` and `BEVControlNetModel` keep the reference's constructor kwargs, parameter names
 (so `load_state_dict(reference.state_dict())` and the diffusers `save_pretrained` directories load unchanged),
@@ -18,7 +18,7 @@ import torch
 import torch.nn as nn
 
 from . import arch, ops
-from .engine import ControlNetEngine, UNetEngine, VaeDecoderEngine
+from .engine import ControlNetEngine, TextEncoderEngine, UNetEngine, VaeDecoderEngine
 
 BF16, F32 = torch.bfloat16, torch.float32
 
@@ -503,3 +503,112 @@ class AutoencoderKL(_B200Module):
             graph.replay()
             img = out.clone()
         return img.reshape(b, n_cam, *img.shape[1:])
+
+
+class CLIPTextModelOutput:  # transformers modeling_outputs.BaseModelOutputWithPooling (last_hidden_state, pooler_output)
+    def __init__(self, last_hidden_state, pooler_output):
+        self.last_hidden_state, self.pooler_output = last_hidden_state, pooler_output
+
+    def __getitem__(self, i):
+        return (self.last_hidden_state, self.pooler_output)[i]
+
+
+class _TextConfig(_Config):
+    """Attribute access like transformers' PretrainedConfig: a missing name is an AttributeError, so that the pipeline's
+    `hasattr(text_encoder.config, "use_attention_mask")` (pipeline_controlnet.py:360) reads False."""
+
+    def __getattr__(self, name):
+        try:
+            return self[name]
+        except KeyError:
+            raise AttributeError(name) from None
+
+
+class CLIPTextModel(_B200Module):
+    """transformers' CLIPTextModel for the pipeline's prompt encoding (pipeline_controlnet.py:365-369, 417-421, called from
+    pipeline_bev_controlnet.py:272) and the box class tokens (BEVControlNetModel.prepare, bbox_embedder.py:123-135): the same
+    constructor (a config or its kwargs), state-dict names (`text_model.*`; the `text_model.embeddings.position_ids` buffer
+    of older checkpoints is accepted and ignored), `from_pretrained(dir, subfolder="text_encoder")` and
+    `forward(input_ids)` returning `.last_hidden_state`, `.pooler_output` and `[0]`.  Runs on TextEncoderEngine; each
+    (batch, length) shape replays one captured CUDA graph.  Padding attention masks are not supported (SD-1.5 sets no
+    `use_attention_mask`, so the pipeline never passes one)."""
+
+    config_name = "config.json"
+    use_cuda_graph = True
+    _graphs: dict = {}
+
+    def __init__(self, config=None, **kwargs):
+        super().__init__()
+        if config is not None:
+            kwargs = {**(config.to_dict() if hasattr(config, "to_dict") else dict(config)), **kwargs}
+        known, extra = _pick(arch.ClipTextConfig, kwargs)
+        cfg = arch.ClipTextConfig(**known)
+        if cfg.hidden_act != "quick_gelu":
+            raise ValueError(f"CLIPTextModel (CUDA): hidden_act {cfg.hidden_act!r} is not implemented (quick_gelu only)")
+        if cfg.hidden_size % cfg.num_attention_heads:
+            raise ValueError("hidden_size must be a multiple of num_attention_heads")
+        self._init_common(cfg, arch.clip_text_param_shapes(cfg), {k: v for k, v in extra.items() if not k.startswith("_")})
+        self.config = _TextConfig(self.config)
+        self.training = False
+
+    def load_state_dict(self, state_dict, strict=True, **kw):
+        sd = {k: v for k, v in state_dict.items() if k != "text_model.embeddings.position_ids"}
+        return super().load_state_dict(sd, strict=strict, **kw)
+
+    @classmethod
+    def from_pretrained(cls, path, subfolder=None, torch_dtype=None, **kw):
+        """config.json + model.safetensors or pytorch_model.bin (a transformers `save_pretrained` directory)."""
+        if subfolder:
+            path = os.path.join(path, subfolder)
+        with open(os.path.join(path, cls.config_name)) as f:
+            model = cls(**json.load(f))
+        st = os.path.join(path, "model.safetensors")
+        if os.path.exists(st):
+            from safetensors.torch import load_file
+            sd = load_file(st)
+        else:
+            sd = torch.load(os.path.join(path, "pytorch_model.bin"), map_location="cpu", weights_only=True)
+        model.load_state_dict(sd, strict=True)
+        if torch_dtype is not None:
+            model = model.to(torch_dtype)
+        return model
+
+    def engine(self) -> TextEncoderEngine:
+        eng = self._get_engine(TextEncoderEngine)
+        if getattr(self, "_graphs_for", None) is not eng:  # weights changed -> engine rebuilt -> graphs stale
+            self._graphs, self._graphs_for = {}, eng
+        return eng
+
+    @torch.no_grad()
+    def forward(self, input_ids, attention_mask=None, position_ids=None, output_attentions=None, output_hidden_states=None,
+                return_dict: bool = True):
+        if attention_mask is not None and bool((attention_mask == 0).any()):
+            raise ValueError("CLIPTextModel (CUDA): padding attention masks are not supported")
+        if position_ids is not None or output_attentions or output_hidden_states:
+            raise ValueError("CLIPTextModel (CUDA): position_ids / output_attentions / output_hidden_states are not supported")
+        n, L = input_ids.shape
+        if L > self.arch_cfg.max_position_embeddings:
+            raise ValueError(f"sequence length {L} exceeds max_position_embeddings {self.arch_cfg.max_position_embeddings}")
+        eng = self.engine()
+        ids = input_ids.to(self.device)
+        if not (self.use_cuda_graph and ids.is_cuda):
+            hidden, pooled = eng.forward(ids)
+        else:
+            key = (n, L, ids.dtype)
+            g = self._graphs.get(key)
+            if g is None:
+                idin = ids.clone()
+                eng.forward(idin)  # eager once: packs the weights and sizes the scratch outside the capture
+                torch.cuda.synchronize()
+                graph = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(graph):
+                    out = eng.forward(idin)
+                g = self._graphs[key] = (graph, idin, out)
+            graph, idin, out = g
+            idin.copy_(ids)
+            graph.replay()
+            hidden, pooled = (t.clone() for t in out)
+        hidden, pooled = hidden.to(self.dtype), pooled.to(self.dtype)
+        if not return_dict:
+            return (hidden, pooled)
+        return CLIPTextModelOutput(hidden, pooled)

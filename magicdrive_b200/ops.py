@@ -126,12 +126,12 @@ def gemm_conv(a0: torch.Tensor, w: torch.Tensor, *, n_img: int, h_in: int, w_in:
               ldo: Optional[int] = None, out_f32: bool = False, out_scale: float = 1.0, geglu: bool = False,
               force_block_n: int = 0, force_splits: int = 0, allow_split_k: bool = True, kernel_variant: int = 0,
               ln: Optional["RowStats"] = None, ln_colsum: Optional[torch.Tensor] = None, ln_eps: float = 1e-5,
-              emit_stats: bool = False):
+              emit_stats: bool = False, quick_gelu: bool = False):
     """wgmma GEMM / implicit-GEMM conv (mdb_gemm_conv).  `a0` (and `a1`) are NHWC bf16 buffers whose pixel
     stride is lda* elements; `w` is bf16 [n_out, taps*taps*(c0+c1)].
     ln / ln_colsum: fold a LayerNorm of the rows of `a0` into this GEMM (`ln` = the RowStats the producer of `a0`
     emitted, `w` pre-multiplied by gamma, `bias` = beta-term + bias).  emit_stats: also return the RowStats of the
-    output rows -> (out, RowStats)."""
+    output rows -> (out, RowStats).  quick_gelu: out = y * sigmoid(1.702 y) (CLIP's MLP activation)."""
     global _launches
     _need_cuda(a0, w)
     if h_out is None:
@@ -158,8 +158,8 @@ def gemm_conv(a0: torch.Tensor, w: torch.Tensor, *, n_img: int, h_in: int, w_in:
     d.rowbias_ld = (rowbias.stride(0) if rowbias.shape[0] > 1 else 0) if rowbias is not None else 0  # 1 row = shared by all images
     d.residual, d.ldr = _ptr(residual), ldr
     d.out, d.ldo, d.out_is_f32, d.out_scale = _ptr(out), ldo, int(out_f32), float(out_scale)
-    d.epi_mode = 1 if geglu else 0
-    if allow_split_k and not geglu:
+    d.epi_mode = 1 if geglu else 2 if quick_gelu else 0
+    if allow_split_k and not geglu and not quick_gelu:
         ws = workspace(64 << 20, a0.device)
         d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel()
     else:
@@ -184,7 +184,7 @@ def gemm_conv(a0: torch.Tensor, w: torch.Tensor, *, n_img: int, h_in: int, w_in:
         check(L.mdb_gemm_conv_plan(C.byref(d), plan), "mdb_gemm_conv_plan")
         _prof_end("gemm_conv", 2.0 * pixels * n_out * taps * taps * (c0 + c1), e0,
                   f"M={pixels} N={n_out} K={taps * taps * (c0 + c1)} img={n_img}x{h_out}x{w_out} taps={taps} s={stride} "
-                  f"geglu={int(geglu)} res={int(residual is not None)} | BN={plan[0]} tiles={plan[1]}x{plan[2]}x{plan[3]} "
+                  f"geglu={int(geglu)} qgelu={int(quick_gelu)} res={int(residual is not None)} | BN={plan[0]} tiles={plan[1]}x{plan[2]}x{plan[3]} "
                   f"waves={plan[4]}")
     _launches += L.mdb_gemm_conv_launches(C.byref(d))
     return (out, stats) if emit_stats else out
@@ -292,6 +292,38 @@ def attention_multi(q, sources, *, b, heads, lq, lk, d, ldq, scale, kv_index, n_
     _prof_end("attention", 4.0 * b * heads * lq * lk * d * n_sets, e0, f"B={b} H={heads} Lq={lq} Lk={lk} D={d} sets={n_sets} src={n}")
     _launches += 1
     return out
+
+
+def attention_causal(q, k, v, *, b, heads, l, d, ldq, ldk, ldv, scale, out=None):
+    """Causal self-attention (mdb_attention_causal): key j is visible to query i iff j <= i.  q/k/v: [b*l, >=heads*d]
+    views with row strides ldq/ldk/ldv; returns [b*l, heads*d] bf16."""
+    global _launches
+    _need_cuda(q, k, v)
+    if out is None:
+        out = torch.empty((b * l, heads * d), dtype=BF16, device=q.device)
+    e0 = _prof_begin()
+    check(_lib.lib().mdb_attention_causal(_ptr(q), ldq, _ptr(k), ldk, _ptr(v), ldv, _ptr(out), out.stride(0), b, heads, l, l, d,
+                                          float(scale), _stream()), "mdb_attention_causal")
+    _prof_end("attention", 2.0 * b * heads * l * (l + 1) * d, e0, f"B={b} H={heads} L={l} D={d} causal")
+    _launches += 1
+    return out
+
+
+def clip_embed(ids, tok, pos, out=None):
+    """CLIP token + position embedding (mdb_clip_embed): ids int32/int64 [n_seq, len] on the device, tok bf16 [vocab, dim],
+    pos bf16 [>= len, dim] -> (bf16 [n_seq*len, dim] residual stream, its RowStats with one part)."""
+    global _launches
+    _need_cuda(ids, tok, pos)
+    n_seq, ln = ids.shape
+    dim = tok.shape[1]
+    assert ids.dtype in (torch.int32, torch.int64) and ids.is_contiguous() and pos.shape[0] >= ln
+    if out is None:
+        out = torch.empty((n_seq * ln, dim), dtype=BF16, device=ids.device)
+    stats = RowStats(torch.empty((n_seq * ln, 1, 2), dtype=F32, device=ids.device), 1)
+    check(_lib.lib().mdb_clip_embed(_ptr(ids), int(ids.dtype == torch.int64), n_seq, ln, _ptr(tok), tok.shape[0], _ptr(pos), dim,
+                                    _ptr(out), out.stride(0), _ptr(stats.data), _stream()), "mdb_clip_embed")
+    _launches += 1
+    return out, stats
 
 
 def peer_barrier(flag_ptrs_dev: int, rank: int, world: int, channel: int, n_channels: int, epoch, timed_out,

@@ -136,22 +136,25 @@ class UniPCSchedule:
 
 
 class BEVControlNetDenoiser:
-    """Call-compatible core of StableDiffusionBEVControlNetPipeline for `output_type="latent"` with precomputed
-    prompt embeddings (the CLIP text encoder and the VAE sit outside the hot path: SURVEY.md §2.1)."""
+    """Call-compatible core of StableDiffusionBEVControlNetPipeline: captions (with a models.CLIPTextModel) or precomputed
+    prompt embeddings in, latents (or, with a models.AutoencoderKL, images) out."""
 
     def __init__(self, unet: UNet2DConditionModelMultiview, controlnet: BEVControlNetModel, use_cuda_graph: bool = True,
                  overlap_controlnet: bool = True, view_shard=None, scheduler: str = "ddim", vae=None,
-                 cfg_streams: bool = False):
+                 cfg_streams: bool = False, text_encoder=None, tokenizer=None):
         """view_shard: a dist.ShardContext to spread each scene's guidance halves x camera views over the ranks of the job
         (inputs are still passed in full on every rank; the result is gathered back to (S, n_cam, ...)).
         scheduler: "ddim" (eta = 0) or "unipc" (the reference's default sampler, misc/test_utils.py:129).
         vae: a models.AutoencoderKL; enables output_type "pt" / "np" (decode_latents, pipeline_bev_controlnet.py:100-112).
+        text_encoder / tokenizer: a models.CLIPTextModel and a transformers CLIPTokenizer; enable `prompt=` /
+        `negative_prompt=` captions in place of precomputed embeddings (_encode_prompt, pipeline_controlnet.py:285-430).
         cfg_streams (opt-in, not yet measured): run the unconditional and the conditional half of the guidance batch as
         two concurrent branches (ControlNet -> UNet each) instead of ControlNet || UNet-encoder on the whole batch, so
         every kernel's fixed cost is overlapped by the other half's kernels; same arithmetic per sample."""
         if scheduler not in ("ddim", "unipc"):
             raise ValueError(f"scheduler must be 'ddim' or 'unipc', got {scheduler!r}")
         self.unet, self.controlnet, self.vae = unet, controlnet, vae
+        self.text_encoder, self.tokenizer = text_encoder, tokenizer
         self.overlap_controlnet = overlap_controlnet
         # programmatic dependent launch on the single-stream UNet up path (A/B switch until measured: MDB_PDL_DECODER=1)
         self.pdl_decoder = os.environ.get("MDB_PDL_DECODER", "0") == "1"
@@ -514,19 +517,62 @@ class BEVControlNetDenoiser:
                 self._graph, self._graph_key, self._graph_state = g, key, st
             self._graph.replay()
 
+    def _encode(self, captions):
+        ids = self.tokenizer(captions, padding="max_length", max_length=self.tokenizer.model_max_length, truncation=True,
+                             return_tensors="pt").input_ids
+        return self.text_encoder(ids.to(self.text_encoder.device))[0]
+
     @torch.no_grad()
-    def __call__(self, image, camera_param, prompt_embeds, negative_prompt_embeds=None, latents=None,
+    def encode_prompt(self, prompt, negative_prompt, prompt_embeds, negative_prompt_embeds, cfg: bool):
+        """_encode_prompt (pipeline_controlnet.py:285-430) with num_images_per_prompt = 1: captions -> text-encoder hidden
+        states, and the unconditional half ("" per scene unless negative_prompt is given) when guidance is on.  The
+        embeddings stay on the text encoder's device."""
+        if prompt is not None and not isinstance(prompt, (str, list)):
+            raise ValueError(f"`prompt` has to be of type `str` or `list` but is {type(prompt)}")
+        needs_encoder = prompt_embeds is None or (cfg and negative_prompt_embeds is None)
+        if needs_encoder and (self.text_encoder is None or self.tokenizer is None):
+            raise ValueError("captions need the denoiser to be built with text_encoder= and tokenizer=; otherwise pass prompt_embeds")
+        batch_size = 1 if isinstance(prompt, str) else len(prompt) if prompt is not None else prompt_embeds.shape[0]
+        if prompt_embeds is None:
+            prompt_embeds = self._encode(prompt)
+        if cfg and negative_prompt_embeds is None:
+            if negative_prompt is None:
+                uncond = [""] * batch_size
+            elif prompt is not None and type(prompt) is not type(negative_prompt):
+                raise TypeError(f"`negative_prompt` should be the same type to `prompt`, but got {type(negative_prompt)} !="
+                                f" {type(prompt)}.")
+            elif isinstance(negative_prompt, str):
+                uncond = [negative_prompt]
+            elif batch_size != len(negative_prompt):
+                raise ValueError(f"`negative_prompt`: {negative_prompt} has batch size {len(negative_prompt)}, but `prompt`:"
+                                 f" {prompt} has batch size {batch_size}. Please make sure that passed `negative_prompt` matches"
+                                 " the batch size of `prompt`.")
+            else:
+                uncond = negative_prompt
+            negative_prompt_embeds = self._encode(uncond)
+        return prompt_embeds, negative_prompt_embeds
+
+    @torch.no_grad()
+    def __call__(self, image, camera_param, prompt_embeds=None, negative_prompt_embeds=None, latents=None,
                  num_inference_steps: int = 50, guidance_scale: float = 2.0, bev_controlnet_kwargs: Optional[Dict] = None,
                  controlnet_conditioning_scale: float = 1.0, output_type: str = "latent", conditional_latents=None,
                  conditional_latents_change_every_input: bool = True, use_zero_map_as_unconditional: bool = False,
                  bbox_max_length: Optional[int] = None, height: Optional[int] = None, width: Optional[int] = None,
-                 generator: Optional[torch.Generator] = None):
+                 generator: Optional[torch.Generator] = None, prompt=None, negative_prompt=None):
         """Same argument meaning as the reference pipeline call (:114-160); with `conditional_latents` it is the
-        given-view pipeline's call (pipeline_bev_controlnet_given_view.py:36-37).  Returns latents (S, n_cam, 4, h, w) fp32."""
+        given-view pipeline's call (pipeline_bev_controlnet_given_view.py:36-37).  Returns latents (S, n_cam, 4, h, w) fp32.
+        `prompt` / `negative_prompt` (a str or one per scene) are encoded by the text encoder when prompt_embeds /
+        negative_prompt_embeds are not given."""
         if output_type not in ("latent", "pt", "np"):
             raise ValueError(f"output_type must be 'latent', 'pt' or 'np', got {output_type!r}")
         if output_type != "latent" and self.vae is None:
             raise ValueError("output_type 'pt' / 'np' needs the denoiser to be built with vae=AutoencoderKL(...)")
+        if prompt is None and prompt_embeds is None:
+            raise ValueError("pass `prompt` or `prompt_embeds`")
+        if prompt is not None or self.text_encoder is not None:
+            # guidance is off without a conditional camera (pipeline_bev_controlnet.py:257-264)
+            prompt_embeds, negative_prompt_embeds = self.encode_prompt(
+                prompt, negative_prompt, prompt_embeds, negative_prompt_embeds, guidance_scale > 1.0 and camera_param is not None)
         boxes = (bev_controlnet_kwargs or {}).get("bboxes_3d_data")
         self.generator = generator
         ss = self.unet.arch_cfg.sample_size * 8  # the reference's default height / width (pipeline_controlnet.py: sample_size * vae_scale_factor)
