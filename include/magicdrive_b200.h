@@ -126,13 +126,16 @@ int mdb_softmax_rows(const float* s, int lds, long long rows, int cols, void* ou
 
 /* Fused multi-head attention forward, softmax(Q K^T * scale) V, bf16 in/out, fp32 softmax.
  * q: [b, Lq, heads*d] with row stride ldq; k, v: [b_kv, Lk, heads*d] with row strides ldk, ldv; out like q (ldo).
- * kv_index: device int32 [b * n_sets] of K/V batch indices (< b_kv) or NULL (then b_kv == b and batch i attends to
- * K/V batch i).  b_kv > b is the view-sharded case: K/V of all views were all-gathered, queries are local.
- * With n_sets == 2 the kernel computes
- *   out[b] = attn(q[b], kv[kv_index[2b]]) + attn(q[b], kv[kv_index[2b+1]])
- * which is the cross-view "add" mode (magicdrive/networks/blocks.py:112-121, 213-217) without the 2x token
- * duplication.  Replaces xformers efficient_attention_forward_cutlass / F.scaled_dot_product_attention
+ * kv_index: device int32 [b * n_sets] of K/V batch indices (< b_kv) or NULL (then n_sets == 1, b_kv == b and batch i attends
+ * to K/V batch i).  b_kv > b is the view-sharded case: K/V of all views were all-gathered, queries are local.
+ * With n_sets in 1..MDB_ATT_MAX_SETS the kernel computes
+ *   out[b] = sum over s with kv_index[b*n_sets + s] >= 0, in order s = 0, 1, ..., of bf16(attn(q[b], kv[kv_index[b*n_sets + s]]))
+ * (each set's output rounded to bf16 before it is added; a row with no entry >= 0 is written as zeros).  An entry -1 is an
+ * empty slot: nothing is loaded for it, so [a, -1, b] gives bitwise the result of [a, b].  This is the cross-view "add" mode
+ * (magicdrive/networks/blocks.py:112-121, 213-217) for any camera rig, without duplicating tokens per (view, neighbour)
+ * pair.  Replaces xformers efficient_attention_forward_cutlass / F.scaled_dot_product_attention
  * (attention_processor.py:1165-1171, 1252). */
+#define MDB_ATT_MAX_SETS 8
 int mdb_attention(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, void* out, int ldo, int b,
                   int b_kv, int heads, int lq, int lk, int d, const int* kv_index, int n_sets, float scale, void* stream);
 
@@ -143,6 +146,15 @@ int mdb_attention(const void* q, int ldq, const void* k, int ldk, const void* v,
 int mdb_attention_multi(const void* q, int ldq, int n_src, const void* const* k, const int* ldk, const void* const* v,
                         const int* ldv, const int* b_kv, void* out, int ldo, int b, int heads, int lq, int lk, int d,
                         const int* kv_index, int n_sets, float scale, void* stream);
+
+/* mdb_attention_multi with a per-query-batch key count: kv_len is a device int32 [b] array or NULL (= lk for every batch).
+ * Keys at or beyond kv_len[b] take no weight and key tiles past it are not loaded.  The kernel clamps each entry to [0, lk]
+ * (a batch with 0 keys contributes nothing, like an empty slot).  This is the cross-view "concat" mode
+ * (blocks.py:122-133) when views have different neighbour counts: their neighbours' tokens are gathered into
+ * [b, lk, heads*d] with kv_len[b] = neighbours * tokens. */
+int mdb_attention_varlen(const void* q, int ldq, int n_src, const void* const* k, const int* ldk, const void* const* v,
+                         const int* ldv, const int* b_kv, void* out, int ldo, int b, int heads, int lq, int lk, int d,
+                         const int* kv_index, int n_sets, const int* kv_len, float scale, void* stream);
 
 /* Causal self-attention of the CLIP text encoder (transformers models/clip/modeling_clip.py CLIPAttention.forward with the
  * causal_attention_mask of CLIPTextTransformer.forward): as mdb_attention with one set, b_kv == b and no kv_index, and key j

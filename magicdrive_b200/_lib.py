@@ -50,7 +50,8 @@ SIGNATURES = {
     "mdb_layernorm": (_i, [_vp, _ll, _i, _i, _vp, _vp, _f, _vp, _i, _vp]),
     "mdb_attention": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _f, _vp]),
     "mdb_attention_multi": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _f, _vp]),
-    "mdb_attention_causal": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _f, _vp]),
+    "mdb_attention_varlen": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _f, _vp]),
+    "mdb_attention_causal":(_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _f, _vp]),
     "mdb_clip_embed": (_i, [_vp, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _vp]),
     "mdb_add": (_i, [_vp, _vp, _vp, _ll, _vp]),
     "mdb_upsample_nearest": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp]),

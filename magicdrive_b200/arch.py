@@ -13,6 +13,24 @@ from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Tuple
 
 DEFAULT_NEIGHBORS = {0: [5, 1], 1: [0, 2], 2: [1, 3], 3: [2, 4], 4: [3, 5], 5: [4, 0]}
+ATT_MAX_SETS = 8  # MDB_ATT_MAX_SETS (include/magicdrive_b200.h): neighbours one view's cross-view attention may sum
+
+
+def check_neighbors(nb: Dict[int, List[int]], attn_type: str) -> None:
+    """Raise ValueError, naming the view, for a camera rig the cross-view attention cannot run: the keys of
+    `neighboring_view_pair` must be exactly the views 0..n_cam-1, every neighbour one of them, at most ATT_MAX_SETS
+    neighbours per view, and none empty under "concat" (the reference's torch.cat of no tensors fails there too)."""
+    n_cam = len(nb)
+    if sorted(nb) != list(range(n_cam)):
+        raise ValueError(f"neighboring_view_pair keys must be the views 0..{n_cam - 1}, got {sorted(nb)}")
+    for view, values in nb.items():
+        bad = [x for x in values if not 0 <= x < n_cam]
+        if bad:
+            raise ValueError(f"neighboring_view_pair[{view}]: neighbour(s) {bad} outside the views 0..{n_cam - 1}")
+        if len(values) > ATT_MAX_SETS:
+            raise ValueError(f"neighboring_view_pair[{view}] lists {len(values)} neighbours; at most {ATT_MAX_SETS} are supported")
+        if not values and attn_type == "concat":
+            raise ValueError(f"neighboring_view_pair[{view}] is empty: neighboring_attn_type 'concat' needs a neighbour per view")
 
 
 @dataclass

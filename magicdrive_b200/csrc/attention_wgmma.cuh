@@ -7,8 +7,12 @@
 //                        A fragment of the next product (no shared-memory round trip)
 //     O = O*corr + P V   wgmma RS  (A = P from registers, B = V tile MN-major straight from the [keys, d] layout)
 //   warp 8: TMA producer (Q per query tile, K/V ring of STAGES), warps 0..7: two consumer warpgroups of 64 query rows each.
-//   n_sets = 2 runs the loop twice against two KV batches (cross-view neighbours) and sums the two normalised outputs
-//   (each rounded to bf16 first, like the reference's per-branch outputs).
+//   n_sets > 1 runs the loop once per KV batch (cross-view neighbours) and sums the normalised outputs in slot order (each
+//   rounded to bf16 first, like the reference's per-branch outputs).  A kv_index entry < 0 is an empty slot: the producer
+//   loads nothing for it and the consumers skip it, both deciding from tiles_of(kv_entry(set), q0); a row with no present
+//   set is written as zeros.
+//   kv_len (optional, per query batch): keys at or beyond min(max(kv_len[b], 0), lk) take no weight and key tiles wholly past
+//   that count are neither loaded nor walked (the "concat" mode with uneven neighbour counts).
 //   Multi-Q mode (p.q_step > 0): the CTA walks the query tiles blockIdx.x, blockIdx.x + q_step, ... of its (batch, head);
 //   with a single K/V tile (lk <= BN, one set: the text / camera / box cross-attention) that tile is loaded once.
 //   CAUSAL (self-attention with lq == lk, one set): key j is visible to query i iff j <= i.  A query tile walks only the key
@@ -33,8 +37,9 @@ struct AttnParams {
   __nv_bfloat16* out;
   int ldo;
   int lq, lk;
-  const int* kv_index;
+  const int* kv_index;  // [b, n_sets]: (source << 24) | batch, or < 0 for an empty slot; nullptr = batch b, one set
   int n_sets;
+  const int* kv_len;    // [b] keys of each query batch's K/V (clamped to [0, lk]); nullptr = lk
   int n_src;
   float scale_log2;
   int q_step;  // > 0: query tiles per CTA walk stride (multi-Q mode); 0 = one query tile per CTA
@@ -80,14 +85,10 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int b = blockIdx.z, head = blockIdx.y;
-  const int ntiles = (p.lk + BN - 1) / BN;
   const int nq = (p.lq + ATT_BM - 1) / ATT_BM;
   const int q_step = p.q_step > 0 ? p.q_step : nq;
   const int n_own = (nq - static_cast<int>(blockIdx.x) + q_step - 1) / q_step;  // query tiles of this CTA
-  const bool kv_resident = ntiles == 1 && p.n_sets == 1 && n_own > 1;
   auto q0_of = [&](int o) { return (static_cast<int>(blockIdx.x) + o * q_step) * ATT_BM; };
-  // key tiles a query tile starting at q0 reads: causal tiles stop at the one holding key min(q0 + ATT_BM, lq) - 1
-  auto tiles_of = [&](int q0) { return CAUSAL ? min(ntiles, (min(q0 + ATT_BM, p.lq) - 1) / BN + 1) : ntiles; };
 
   if (warp == Cfg::kConsumerWarps && lane == 0) {
     prefetch_tmap(&tmQ);
@@ -106,6 +107,16 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
   __syncthreads();
   asm volatile("griddepcontrol.wait;" ::: "memory");  // PDL: prologue above overlapped the predecessor's tail
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  // kv_index / kv_len may be written by the predecessor kernel: read only after the PDL wait
+  const int lkb = p.kv_len ? min(max(p.kv_len[b], 0), p.lk) : p.lk;  // keys of this batch; the maps never go past lk
+  const int ntiles = (lkb + BN - 1) / BN;
+  const bool kv_resident = ntiles == 1 && p.n_sets == 1 && n_own > 1;
+  auto kv_entry = [&](int set) { return p.kv_index ? p.kv_index[b * p.n_sets + set] : b; };
+  // key tiles the set with kv_index entry kve reads for the query tile starting at q0: none for an empty slot; causal tiles
+  // stop at the one holding key min(q0 + ATT_BM, lq) - 1.  Producer and consumers both take their counts from here.
+  auto tiles_of = [&](int kve, int q0) {
+    return kve < 0 ? 0 : CAUSAL ? min(ntiles, (min(q0 + ATT_BM, p.lq) - 1) / BN + 1) : ntiles;
+  };
 
   if (warp == Cfg::kConsumerWarps) {
     // =========================== TMA producer ===========================
@@ -119,11 +130,12 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
         for (int c = 0; c < KD; ++c) tma_load_4d(&tmQ, q_full, smQ + c * TILE_Q, c * 64, head, q0_of(o), b);
         if (kv_resident && o > 0) continue;
         for (int set = 0; set < p.n_sets; ++set) {
-          const int kve = p.kv_index ? p.kv_index[b * p.n_sets + set] : b;
+          const int kve = kv_entry(set);
+          const int nt = tiles_of(kve, q0_of(o));
+          if (nt == 0) continue;
           const int kvb = kve & 0xffffff;
           const CUtensorMap* km = &kvm.k[kve >> 24];
           const CUtensorMap* vm = &kvm.v[kve >> 24];
-          const int nt = tiles_of(q0_of(o));
           for (int j = 0; j < nt; ++j) {
             mbar_wait(&kv_empty[stage], phase ^ 1);
             mbar_arrive_expect_tx(&kv_full[stage], 2 * KD * TILE_KV);
@@ -153,12 +165,14 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
   for (int o = 0; o < n_own; ++o) {
     const int q0 = q0_of(o);
     mbar_wait(q_full, static_cast<uint32_t>(o) & 1u);
+    bool wrote = false;  // a present set was stored to this query tile's rows (uniform over the CTA)
     for (int set = 0; set < p.n_sets; ++set) {
+      const int nt = tiles_of(kv_entry(set), q0);
+      if (nt == 0) continue;
       float oacc[Cfg::OACC];
 #pragma unroll
       for (int i = 0; i < Cfg::OACC; ++i) oacc[i] = 0.f;
       float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
-      const int nt = tiles_of(q0);
       for (int j = 0; j < nt; ++j) {
         const int st = kv_resident ? 0 : stage;
         mbar_wait(&kv_full[st], kv_resident ? 0u : phase);
@@ -174,14 +188,14 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
         }
         wgmma_commit();
         wgmma_wait<0>();
-        // ---- keys past lk (zero-filled by TMA) take no weight
+        // ---- keys past this batch's key count (past lk: zero-filled by TMA) take no weight
         const int kbase = j * BN;
-        if (kbase + BN > p.lk) {
+        if (kbase + BN > lkb) {
 #pragma unroll
           for (int g = 0; g < BN / 8; ++g)
 #pragma unroll
             for (int e = 0; e < 2; ++e)
-              if (kbase + 8 * g + 2 * q + e >= p.lk) s[4 * g + e] = s[4 * g + 2 + e] = -INFINITY;
+              if (kbase + 8 * g + 2 * q + e >= lkb) s[4 * g + e] = s[4 * g + 2 + e] = -INFINITY;
         }
         // ---- causal: keys after the query row take no weight (only tiles that reach past the tile's first row)
         if constexpr (CAUSAL) {
@@ -264,14 +278,26 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
           const int col = 8 * g + 2 * q;
           if (col >= D) continue;
           float f0 = oacc[4 * g + 2 * h] * inv[h], f1 = oacc[4 * g + 2 * h + 1] * inv[h];
-          if (set > 0) {
-            // both branches rounded to bf16 before the sum, like the reference's per-branch attention outputs
+          if (wrote) {
+            // every branch rounded to bf16 before the sum, like the reference's per-branch attention outputs
             const float2 pf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(orow + col));
             f0 = __bfloat162float(__float2bfloat16_rn(f0)) + pf.x;
             f1 = __bfloat162float(__float2bfloat16_rn(f1)) + pf.y;
           }
           *reinterpret_cast<uint32_t*>(orow + col) = pack_bf16(f0, f1);
         }
+      }
+      wrote = true;
+    }
+    if (!wrote) {  // no present set: the sum over no neighbours is zero
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int qrow = q0 + rloc + 8 * h;
+        if (qrow >= p.lq) continue;
+        __nv_bfloat16* orow = p.out + (static_cast<long long>(b) * p.lq + qrow) * p.ldo + head * D;
+#pragma unroll
+        for (int g = 0; g < D16 / 8; ++g)
+          if (8 * g + 2 * q < D) *reinterpret_cast<uint32_t*>(orow + 8 * g + 2 * q) = 0u;
       }
     }
     __syncwarp();

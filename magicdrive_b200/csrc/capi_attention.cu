@@ -1,9 +1,11 @@
 // Fused multi-head attention forward (flash-style, online softmax in fp32) on wgmma + TMA: C-ABI launchers.
 //
 // Layout: q/out [B, Lq, heads*D] (row strides ldq/ldo), k/v [Bkv, Lk, heads*D] (ldk/ldv): exactly what the fused
-// QKV projection GEMM writes, so no head transpose is ever materialised.  With n_sets == 2 the kernel runs two
-// independent softmaxes against two KV batches and writes their sum: the cross-view "add" mode of
-// BasicMultiviewTransformerBlock (magicdrive/networks/blocks.py:112-121, 213-217).  K/V may be spread over up to three
+// QKV projection GEMM writes, so no head transpose is ever materialised.  With n_sets > 1 the kernel runs one independent
+// softmax per KV batch and writes their sum (empty slots, kv_index < 0, add nothing): the cross-view "add" mode of
+// BasicMultiviewTransformerBlock (magicdrive/networks/blocks.py:112-121, 213-217) for any neighbour count up to
+// MDB_ATT_MAX_SETS.  mdb_attention_varlen also takes a per-batch key count (the "concat" mode with uneven neighbour
+// counts).  K/V may be spread over up to three
 // buffers (mdb_attention_multi): in view-sharded runs the neighbour views' K/V are read in place from the ring-neighbour
 // GPUs' buffers through NVLink peer memory (the tensor maps simply point at peer-mapped addresses).
 // mdb_attention_causal is the CLIP text encoder's masked self-attention (one set, one source, lq == lk).
@@ -80,7 +82,7 @@ int multi_q_step(int b, int heads, int lq, int lk, int n_sets, int bn) {
 
 template <int D, int BN_, bool CAUSAL>
 int launch_attention(const void* q, int ldq, const KvSources& src, void* out, int ldo, int b, int heads, int lq, int lk,
-                     const int* kv_index, int n_sets, float scale, cudaStream_t st) {
+                     const int* kv_index, int n_sets, const int* kv_len, float scale, cudaStream_t st) {
   using Cfg = mdb::AttnCfg<D, BN_>;
   static bool attr = false;
   if (!attr) {
@@ -94,7 +96,7 @@ int launch_attention(const void* q, int ldq, const KvSources& src, void* out, in
     return mdb::set_error(MDB_ERR_CUDA, "mdb_attention: cuTensorMapEncodeTiled failed (d=%d heads=%d lq=%d lk=%d)", D, heads, lq, lk);
   mdb::AttnParams p;
   p.out = static_cast<__nv_bfloat16*>(out);
-  p.ldo = ldo, p.lq = lq, p.lk = lk, p.kv_index = kv_index, p.n_sets = n_sets, p.n_src = src.n;
+  p.ldo = ldo, p.lq = lq, p.lk = lk, p.kv_index = kv_index, p.n_sets = n_sets, p.kv_len = kv_len, p.n_src = src.n;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.q_step = multi_q_step(b, heads, lq, lk, n_sets, Cfg::BN);
   dim3 grid(p.q_step > 0 ? p.q_step : (lq + mdb::ATT_BM - 1) / mdb::ATT_BM, heads, b);
@@ -107,13 +109,13 @@ int launch_attention(const void* q, int ldq, const KvSources& src, void* out, in
 
 template <int BN_, bool CAUSAL>
 int attention_dispatch_bn(const void* q, int ldq, const KvSources& src, void* out, int ldo, int b, int heads, int lq, int lk, int d,
-                          const int* kv_index, int n_sets, float scale, cudaStream_t st) {
+                          const int* kv_index, int n_sets, const int* kv_len, float scale, cudaStream_t st) {
   switch (d) {
-    case 32: return launch_attention<32, BN_, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
-    case 40: return launch_attention<40, BN_, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
-    case 64: return launch_attention<64, BN_, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
-    case 80: return launch_attention<80, BN_, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
-    case 160: return launch_attention<160, BN_, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, scale, st);
+    case 32: return launch_attention<32, BN_, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, kv_len, scale, st);
+    case 40: return launch_attention<40, BN_, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, kv_len, scale, st);
+    case 64: return launch_attention<64, BN_, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, kv_len, scale, st);
+    case 80: return launch_attention<80, BN_, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, kv_len, scale, st);
+    case 160: return launch_attention<160, BN_, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, kv_len, scale, st);
     default: return mdb::set_error(MDB_ERR_UNSUPPORTED, "mdb_attention: head dim %d not instantiated (32, 40, 64, 80, 160)", d);
   }
 }
@@ -122,25 +124,25 @@ int attention_dispatch_bn(const void* q, int ldq, const KvSources& src, void* ou
 // tc2d (64-key tiles: smaller S fragment, deeper K/V ring) | tc (128-key tiles for every head dim).
 template <bool CAUSAL = false>
 int attention_dispatch(const void* q, int ldq, const KvSources& src, void* out, int ldo, int b, int heads, int lq, int lk, int d,
-                       const int* kv_index, int n_sets, float scale, cudaStream_t st) {
+                       const int* kv_index, int n_sets, const int* kv_len, float scale, cudaStream_t st) {
   const char* e = getenv("MDB_ATTN_KERNEL");
-  if (e && !strcmp(e, "tc2d")) return attention_dispatch_bn<64, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, scale, st);
-  if (e && !strcmp(e, "tc")) return attention_dispatch_bn<128, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, scale, st);
+  if (e && !strcmp(e, "tc2d")) return attention_dispatch_bn<64, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, kv_len, scale, st);
+  if (e && !strcmp(e, "tc")) return attention_dispatch_bn<128, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, kv_len, scale, st);
   if (e && *e && strcmp(e, "tc2"))
     return mdb::set_error(MDB_ERR_INVALID, "mdb_attention: MDB_ATTN_KERNEL must be tc2, tc2d or tc (got %s)", e);
-  return attention_dispatch_bn<0, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, scale, st);
+  return attention_dispatch_bn<0, CAUSAL>(q, ldq, src, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, kv_len, scale, st);
 }
 
 }  // namespace
 
-extern "C" int mdb_attention_multi(const void* q, int ldq, int n_src, const void* const* k, const int* ldk, const void* const* v,
-                                   const int* ldv, const int* b_kv, void* out, int ldo, int b, int heads, int lq, int lk, int d,
-                                   const int* kv_index, int n_sets, float scale, void* stream) {
+extern "C" int mdb_attention_varlen(const void* q, int ldq, int n_src, const void* const* k, const int* ldk, const void* const* v,
+                                    const int* ldv, const int* b_kv, void* out, int ldo, int b, int heads, int lq, int lk, int d,
+                                    const int* kv_index, int n_sets, const int* kv_len, float scale, void* stream) {
   using namespace mdb;
   if (!q || !k || !v || !ldk || !ldv || !b_kv || !out) return set_error(MDB_ERR_INVALID, "mdb_attention: null pointer");
   if (n_src < 1 || n_src > ATT_MAX_SRC) return set_error(MDB_ERR_INVALID, "mdb_attention: 1..%d K/V sources", ATT_MAX_SRC);
-  if (n_sets < 1 || n_sets > 2 || (n_sets == 2 && !kv_index))
-    return set_error(MDB_ERR_INVALID, "mdb_attention: n_sets must be 1 or 2 (2 needs kv_index)");
+  if (n_sets < 1 || n_sets > MDB_ATT_MAX_SETS || (n_sets > 1 && !kv_index))
+    return set_error(MDB_ERR_INVALID, "mdb_attention: n_sets must be 1..%d (more than 1 needs kv_index)", MDB_ATT_MAX_SETS);
   if (scale <= 0.f) return set_error(MDB_ERR_INVALID, "mdb_attention: scale must be positive");
   if (lq <= 0 || lk <= 0 || b <= 0 || heads <= 0) return set_error(MDB_ERR_INVALID, "mdb_attention: bad shape");
   if (ldq % 8 || ldo % 8) return set_error(MDB_ERR_UNSUPPORTED, "mdb_attention: strides must be multiples of 8");
@@ -152,7 +154,15 @@ extern "C" int mdb_attention_multi(const void* q, int ldq, int n_src, const void
     src.k[i] = k[i], src.v[i] = v[i], src.ldk[i] = ldk[i], src.ldv[i] = ldv[i], src.b_kv[i] = b_kv[i];
   }
   if (!kv_index && (n_src != 1 || b_kv[0] != b)) return set_error(MDB_ERR_INVALID, "mdb_attention: b_kv != b or several sources need kv_index");
-  return attention_dispatch(q, ldq, src, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, scale, static_cast<cudaStream_t>(stream));
+  return attention_dispatch(q, ldq, src, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, kv_len, scale,
+                            static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int mdb_attention_multi(const void* q, int ldq, int n_src, const void* const* k, const int* ldk, const void* const* v,
+                                   const int* ldv, const int* b_kv, void* out, int ldo, int b, int heads, int lq, int lk, int d,
+                                   const int* kv_index, int n_sets, float scale, void* stream) {
+  return mdb_attention_varlen(q, ldq, n_src, k, ldk, v, ldv, b_kv, out, ldo, b, heads, lq, lk, d, kv_index, n_sets, nullptr, scale,
+                              stream);
 }
 
 extern "C" int mdb_attention(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, void* out, int ldo, int b,
@@ -172,5 +182,6 @@ extern "C" int mdb_attention_causal(const void* q, int ldq, const void* k, int l
   KvSources src;
   src.n = 1;
   src.k[0] = k, src.v[0] = v, src.ldk[0] = ldk, src.ldv[0] = ldv, src.b_kv[0] = b;
-  return attention_dispatch<true>(q, ldq, src, out, ldo, b, heads, lq, lk, d, nullptr, 1, scale, static_cast<cudaStream_t>(stream));
+  return attention_dispatch<true>(q, ldq, src, out, ldo, b, heads, lq, lk, d, nullptr, 1, nullptr, scale,
+                                  static_cast<cudaStream_t>(stream));
 }

@@ -106,6 +106,9 @@ class ShardPlan:
     def __init__(self, rank: int, world: int, n_cam: int, cfg: bool, pairs: Sequence[Sequence[int]]):
         if world < 1 or not 0 <= rank < world:
             raise ValueError(f"bad rank/world {rank}/{world}")
+        if len(pairs) != n_cam or any(len(p) != 2 for p in pairs):
+            raise ValueError("splitting the views across GPUs needs a rig where every view has exactly two neighbours "
+                             f"(got {[list(p) for p in pairs]} for {n_cam} views)")
         self.rank, self.world, self.n_cam, self.cfg = rank, world, n_cam, cfg
         self.split_cfg = bool(cfg and world % 2 == 0)
         self.groups = world // 2 if self.split_cfg else world        # ranks sharing the views of one half

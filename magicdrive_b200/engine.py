@@ -7,7 +7,7 @@ Dataflow differs from the reference on purpose (GPU-first), results do not:
     read two sources;
   * self / cross-view attention use one fused QKV GEMM; cross-view attention reads the neighbours' K/V in place
     (kv_index) instead of duplicating every view's tokens twice (blocks.py:113-121) and `connector(to_out(.))`
-    is folded into one GEMM: Wc(Wo(o_l + o_r) + 2 b_o) + b_c  (blocks.py:203-222);
+    is folded into one GEMM: Wc(Wo(o_1 + ... + o_k) + k b_o) + b_c for a view with k neighbours (blocks.py:203-222);
   * everything that does not depend on the latents is hoisted out of the step: text-context K/V projections,
     camera / box tokens, the BEV-map encoder (computed once per scene, not per view per step), and all 22+10
     `time_emb_proj` linears run as one skinny GEMM.
@@ -144,6 +144,17 @@ class _Weights:
             self.t[k + ".b"] = _f32(float(bias_count) * (wc @ bo) + bc)
         return self.t[k + ".w"], self.t[k + ".b"]
 
+    def connector_rowbias(self, blk, counts: List[int]):
+        """[len(counts), C] fp32: row v = counts[v] * Wc b_o + b_c, the folded connector bias of a view that sums counts[v]
+        attention outputs ('add' mode with uneven neighbour counts; the GEMM's per-image rowbias)."""
+        k = blk + ".attn4.rowbias." + ",".join(map(str, counts))
+        if k not in self.t:
+            wc = self.raw(blk + ".connector.weight").float()
+            cb = wc @ self.raw(blk + ".attn4.to_out.0.bias").float()
+            n = torch.tensor(counts, dtype=F32, device=cb.device)
+            self.t[k] = _f32(n[:, None] * cb[None, :] + self.raw(blk + ".connector.bias").float()[None, :])
+        return self.t[k]
+
 
 class _Net:
     """Shared machinery of the UNet and the ControlNet encoder."""
@@ -214,9 +225,11 @@ class _Net:
         return FMap(out, x.n, x.h, x.w, rs.cout)
 
     def kv_index(self, n_views: int) -> torch.Tensor:
-        """[V, 2] int32: the two ring neighbours of each view inside its own scene (Nuscenes.yaml:27-33).  With the views
-        split across GPUs (dist.ShardContext) an entry is (source << 24) | batch, source 0 = this GPU's K/V buffer,
-        1 / 2 = the ring-neighbour GPUs' buffers (mdb_attention_multi)."""
+        """[V, kmax] int32: the neighbours of each view inside its own scene in `neighboring_view_pair` order, padded with -1
+        (an empty slot of mdb_attention) up to kmax, the largest neighbour count (at least 1).  The nuScenes ring
+        (Nuscenes.yaml:27-33) gives [V, 2] without padding.  With the views split across GPUs (dist.ShardContext, two
+        neighbours per view) an entry is (source << 24) | batch, source 0 = this GPU's K/V buffer, 1 / 2 = the
+        ring-neighbour GPUs' buffers (mdb_attention_multi)."""
         if n_views not in self._kv_idx:
             nb = self.cfg.neighboring_view_pair
             n_cam = len(nb)
@@ -227,9 +240,24 @@ class _Net:
                 idx = [[idx[2 * i], idx[2 * i + 1]] for i in range(n_views)]
             else:
                 assert n_views % n_cam == 0
-                idx = [[s * n_cam + nb[i][0], s * n_cam + nb[i][1]] for s in range(n_views // n_cam) for i in range(n_cam)]
+                kmax = max(1, max(len(v) for v in nb.values()))
+                idx = [[s * n_cam + x for x in nb[i]] + [-1] * (kmax - len(nb[i]))
+                       for s in range(n_views // n_cam) for i in range(n_cam)]
             self._kv_idx[n_views] = torch.tensor(idx, dtype=torch.int32, device=self.device)
         return self._kv_idx[n_views]
+
+    def _uniform_neighbors(self) -> bool:
+        return len({len(v) for v in self.cfg.neighboring_view_pair.values()}) == 1
+
+    def kv_len(self, n_views: int, L: int) -> torch.Tensor:
+        """[V] int32 key counts of the "concat" gather when the views have different neighbour counts: k_v * L."""
+        key = ("len", n_views, L)
+        if key not in self._kv_idx:
+            nb = self.cfg.neighboring_view_pair
+            n_cam = len(nb)
+            self._kv_idx[key] = torch.tensor([len(nb[i]) * L for _ in range(n_views // n_cam) for i in range(n_cam)],
+                                             dtype=torch.int32, device=self.device)
+        return self._kv_idx[key]
 
     def _sharded(self) -> bool:
         return self.view_shard is not None and self.view_shard.plan.groups > 1
@@ -319,8 +347,9 @@ class _Net:
                 o = ops.attention(qkv, qkv[:, C:], qkv[:, 2 * C:], b=V // n_cam, heads=heads, lq=n_cam * L, lk=n_cam * L, d=d,
                                   ldq=3 * C, ldk=3 * C, ldv=3 * C, scale=scale)
             elif at == "concat":
-                # blocks.py:122-133: ONE softmax over the keys of both neighbours.  Their K/V rows are gathered into one
-                # [V, n_nb * L, 2C] buffer (a device copy; this non-default mode is not on the benchmarked path)
+                # blocks.py:122-133: ONE softmax over the keys of all listed neighbours.  Their K/V rows are gathered into
+                # one [V, kmax * L, 2C] buffer (a device copy; this non-default mode is not on the benchmarked path); with
+                # uneven neighbour counts the padding slots' keys are cut off by the per-view key count k_v * L
                 wq, cq, sq = W.ln_lin(blk + ".attn4.lnq", blk + ".norm4", [blk + ".attn4.to_q"])
                 wkv, ckv, skv = W.ln_lin(blk + ".attn4.lnkv", blk + ".norm4", [blk + ".attn4.to_k", blk + ".attn4.to_v"])
                 q = ops.linear(X, wq, bias=cq, ln=sx, ln_colsum=sq)
@@ -328,14 +357,17 @@ class _Net:
                 idx = self.kv_index(V)
                 n_nb = idx.shape[1]
                 kvc = kv.view(V, L, 2 * C)[idx.long()].reshape(V * n_nb * L, 2 * C)
+                uneven = {} if self._uniform_neighbors() else {"kv_len": self.kv_len(V, L)}
                 o = ops.attention(q, kvc, kvc[:, C:], b=V, heads=heads, lq=L, lk=n_nb * L, d=d, ldq=C, ldk=2 * C, ldv=2 * C,
-                                  scale=scale)
+                                  scale=scale, **uneven)
             elif not self._sharded():
+                # blocks.py:112-121: one softmax per (view, neighbour) pair, summed per view; padding slots are empty
                 wqkv, cq, sq = W.ln_lin(blk + ".attn4.lnqkv", blk + ".norm4",
                                         [blk + ".attn4.to_q", blk + ".attn4.to_k", blk + ".attn4.to_v"])
                 qkv = ops.linear(X, wqkv, bias=cq, ln=sx, ln_colsum=sq)
+                idx = self.kv_index(V)
                 o = ops.attention(qkv, qkv[:, C:], qkv[:, 2 * C:], b=V, heads=heads, lq=L, lk=L, d=d, ldq=3 * C,
-                                  ldk=3 * C, ldv=3 * C, scale=scale, kv_index=self.kv_index(V), n_sets=2)
+                                  ldk=3 * C, ldv=3 * C, scale=scale, kv_index=idx, n_sets=idx.shape[1])
             else:
                 # cameras split across GPUs: K/V of the local views go to a symmetric buffer; after one device-side
                 # barrier the attention kernel reads the two ring neighbours' K/V tiles IN PLACE from the neighbour
@@ -348,8 +380,17 @@ class _Net:
                 self.view_shard.half_group.barrier(0)
                 o = ops.attention_multi(q, [(t, t[:, C:], 2 * C, vg) for t, vg in srcs], b=V, heads=heads, lq=L, lk=L, d=d,
                                         ldq=C, scale=scale, kv_index=self.kv_index(V), n_sets=2)
-            wf, bf_ = W.folded_connector(blk, bias_count=2 if at == "add" else 1)
-            X, sx = ops.linear(o, wf, bias=bf_, residual=X, emit_stats=True)
+            nb = cfg.neighboring_view_pair
+            if at != "add" or self._uniform_neighbors():
+                wf, bf_ = W.folded_connector(blk, bias_count=len(nb[0]) if at == "add" else 1)
+                X, sx = ops.linear(o, wf, bias=bf_, residual=X, emit_stats=True)
+            else:
+                # views sum different numbers of attention outputs, so the folded bias k_v Wc b_o + b_c differs per view:
+                # one GEMM "image" per view (L token rows) picks its row of the [V, C] table
+                wf, _ = W.folded_connector(blk, bias_count=1)
+                X, sx = ops.gemm_conv(o, wf, n_img=V, h_in=1, w_in=L, c0=C, lda0=o.stride(0), n_out=C,
+                                      rowbias=W.connector_rowbias(blk, [len(nb[i % len(nb)]) for i in range(V)]),
+                                      residual=X, ldr=X.stride(0), emit_stats=True)
         # --- GEGLU feed-forward
         wg, cg, sg = W.ln_lin(blk + ".ff.lnproj", blk + ".norm3", [blk + ".ff.net.0.proj"], geglu=True)
         hg = ops.linear(X, wg, bias=cg, geglu=True, ln=sx, ln_colsum=sg)

@@ -172,6 +172,7 @@ class UNet2DConditionModelMultiview(_B200Module):
         elif "neighboring_view_pair" in known:
             known.pop("neighboring_view_pair")
         cfg = arch.UNetConfig(**known)
+        arch.check_neighbors(cfg.neighboring_view_pair, cfg.neighboring_attn_type)
         for k, want in (("use_linear_projection", False), ("class_embed_type", None), ("addition_embed_type", None),
                         ("resnet_time_scale_shift", "default"), ("dual_cross_attention", False),
                         ("upcast_attention", False), ("center_input_sample", False), ("encoder_hid_dim", None),

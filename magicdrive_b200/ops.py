@@ -258,8 +258,14 @@ def softmax_rows(s, cols: int, cols_out: int):
     return out
 
 
-def attention(q, k, v, *, b, heads, lq, lk, d, ldq, ldk, ldv, scale, kv_index=None, n_sets=1, out=None, b_kv=None):
-    """q: [b*lq, >=heads*d] view with row stride ldq, k/v [b_kv*lk, ...] likewise; returns [b*lq, heads*d] bf16."""
+def attention(q, k, v, *, b, heads, lq, lk, d, ldq, ldk, ldv, scale, kv_index=None, n_sets=1, out=None, b_kv=None,
+              kv_len=None):
+    """q: [b*lq, >=heads*d] view with row stride ldq, k/v [b_kv*lk, ...] likewise; returns [b*lq, heads*d] bf16.
+    kv_index: int32 [b, n_sets] (n_sets <= 8), -1 = empty slot; the sets' outputs are summed.  kv_len: int32 [b] keys per
+    query batch (mdb_attention_varlen), None = lk."""
+    if kv_len is not None:
+        return attention_multi(q, [(k, v, ldk, b if b_kv is None else b_kv, ldv)], b=b, heads=heads, lq=lq, lk=lk, d=d,
+                               ldq=ldq, scale=scale, kv_index=kv_index, n_sets=n_sets, out=out, kv_len=kv_len)
     b_kv = b if b_kv is None else b_kv
     global _launches
     _need_cuda(q, k, v)
@@ -273,22 +279,30 @@ def attention(q, k, v, *, b, heads, lq, lk, d, ldq, ldk, ldv, scale, kv_index=No
     return out
 
 
-def attention_multi(q, sources, *, b, heads, lq, lk, d, ldq, scale, kv_index, n_sets=1, out=None):
-    """Fused attention whose K/V batches live in up to three buffers (mdb_attention_multi).  `sources` = list of (k, v, ld, b_kv):
-    k / v are [b_kv * lk, >= heads*d] views with row stride ld (a peer GPU's buffer mapped through NVLink works like a local
-    one); kv_index entries are (source << 24) | batch index."""
+def attention_multi(q, sources, *, b, heads, lq, lk, d, ldq, scale, kv_index, n_sets=1, out=None, kv_len=None):
+    """Fused attention whose K/V batches live in up to three buffers (mdb_attention_multi).  `sources` = list of (k, v, ld, b_kv)
+    or (k, v, ldk, b_kv, ldv): k / v are [b_kv * lk, >= heads*d] views with row stride ld (a peer GPU's buffer mapped through
+    NVLink works like a local one); kv_index entries are (source << 24) | batch index, or -1 for an empty slot.
+    kv_len: int32 [b] keys per query batch (mdb_attention_varlen), None = lk."""
     global _launches
-    _need_cuda(q, *[t for s_ in sources for t in s_[:2]])
+    _need_cuda(q, *[t for s_ in sources for t in s_[:2]], kv_len)
     n = len(sources)
     if out is None:
         out = torch.empty((b * lq, heads * d), dtype=BF16, device=q.device)
     ks = (C.c_void_p * n)(*[s_[0].data_ptr() for s_ in sources])
     vs = (C.c_void_p * n)(*[s_[1].data_ptr() for s_ in sources])
     ldk = (C.c_int * n)(*[int(s_[2]) for s_ in sources])
+    ldv = (C.c_int * n)(*[int(s_[4] if len(s_) > 4 else s_[2]) for s_ in sources])
     bkv = (C.c_int * n)(*[int(s_[3]) for s_ in sources])
     e0 = _prof_begin()
-    check(_lib.lib().mdb_attention_multi(_ptr(q), ldq, n, ks, ldk, vs, ldk, bkv, _ptr(out), out.stride(0), b, heads, lq, lk, d,
-                                         _ptr(kv_index), n_sets, float(scale), _stream()), "mdb_attention_multi")
+    if kv_len is None:
+        check(_lib.lib().mdb_attention_multi(_ptr(q), ldq, n, ks, ldk, vs, ldv, bkv, _ptr(out), out.stride(0), b, heads, lq, lk,
+                                             d, _ptr(kv_index), n_sets, float(scale), _stream()), "mdb_attention_multi")
+    else:
+        assert kv_len.dtype == torch.int32 and kv_len.numel() == b
+        check(_lib.lib().mdb_attention_varlen(_ptr(q), ldq, n, ks, ldk, vs, ldv, bkv, _ptr(out), out.stride(0), b, heads, lq, lk,
+                                              d, _ptr(kv_index), n_sets, _ptr(kv_len), float(scale), _stream()),
+              "mdb_attention_varlen")
     _prof_end("attention", 4.0 * b * heads * lq * lk * d * n_sets, e0, f"B={b} H={heads} Lq={lq} Lk={lk} D={d} sets={n_sets} src={n}")
     _launches += 1
     return out
