@@ -85,8 +85,9 @@ typedef struct {
   int ln_parts;
   float ln_eps;
   const float* ln_colsum;  /* fp32 [n_out]: sum_k W'[n, k] */
-  /* Producer side: fp32 [pixels, mdb_gemm_conv_stats_parts(d), 2] receiving partial (sum, sum of squares) of every bf16
-   * output row (after bias / residual), or NULL. */
+  /* Producer side: fp32 [pixels, mdb_gemm_conv_stats_parts(d), 2] receiving partial (sum, sum of squares) of every output
+   * row (after bias / residual) over the columns of one N tile per slot, taken from the stored values (bf16-rounded for
+   * bf16 outputs), or NULL. */
   float* stats_out;
 } mdb_gemm_desc;
 

@@ -51,7 +51,8 @@ struct GemmParams {
   int ln_parts;
   float ln_inv_c, ln_eps;
   const float* ln_colsum;  // [n_out] sum_k W'[n, k]
-  // row statistics of this GEMM's output (producer side): [pixels][n_tiles][2] partial (sum, sum sq), or nullptr
+  // row statistics of this GEMM's output (producer side): [pixels][n_tiles][2] partial (sum, sum sq) of the values as
+  // stored (bf16-rounded for bf16 outputs), or nullptr
   float* stats_out;
 };
 

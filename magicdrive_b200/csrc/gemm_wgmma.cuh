@@ -278,12 +278,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
           const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.residual + pix[h] * p.ldr + col));
           v0 += r.x, v1 += r.y;
         }
+        if (p.out_is_f32) {
+          *reinterpret_cast<float2*>(static_cast<float*>(p.out) + pix[h] * p.ldo + col) = make_float2(v0, v1);
+        } else {
+          const uint32_t pk = pack_bf16(v0, v1);
+          *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.out) + pix[h] * p.ldo + col) = pk;
+          // the row statistics describe the values as stored: the consumer's folded LayerNorm multiplies these
+          v0 = __uint_as_float(pk << 16), v1 = __uint_as_float(pk & 0xffff0000u);
+        }
         st_s[h] += v0 + v1;
         st_ss[h] = fmaf(v0, v0, fmaf(v1, v1, st_ss[h]));
-        if (p.out_is_f32)
-          *reinterpret_cast<float2*>(static_cast<float*>(p.out) + pix[h] * p.ldo + col) = make_float2(v0, v1);
-        else
-          *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.out) + pix[h] * p.ldo + col) = pack_bf16(v0, v1);
       }
     }
     if (p.stats_out != nullptr) {

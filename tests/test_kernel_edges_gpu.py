@@ -217,7 +217,7 @@ def test_gemm_m_tails(cuda_lib, n, h, w, taps, stride, variant):
 @pytest.mark.parametrize("variant", VARIANTS, ids=VARIANT_IDS)
 @pytest.mark.parametrize("stats", [False, True], ids=["plain", "stats"])
 @pytest.mark.parametrize("bn", [64, 128, 160, 256])
-@pytest.mark.parametrize("n_out", [8, 40, 136])
+@pytest.mark.parametrize("n_out", [8, 40, 136, 264, 520])  # a tail past every block width
 def test_gemm_n_tails(cuda_lib, n_out, bn, stats, variant):
     g = _gen(4)
     m, k = 1000, 320
@@ -235,9 +235,10 @@ def test_gemm_n_tails(cuda_lib, n_out, bn, stats, variant):
         st = res[1]
         assert st.parts == (n_out + bn - 1) // bn and st.data.shape == (m, st.parts, 2)
         s = st.data.to(F64).sum(1)
-        # the statistics are taken from the fp32 values before their rounding to bf16
-        torch.testing.assert_close(s[:, 0], ref.sum(1), rtol=0, atol=2e-3)
-        torch.testing.assert_close(s[:, 1], (ref ** 2).sum(1), rtol=1e-5, atol=2e-3)
+        # the statistics are taken from the values as stored, after their rounding to bf16
+        stored = out.out.to(F64)
+        torch.testing.assert_close(s[:, 0], stored.sum(1), rtol=0, atol=2e-3)
+        torch.testing.assert_close(s[:, 1], (stored ** 2).sum(1), rtol=1e-5, atol=2e-3)
 
 
 @pytest.mark.parametrize("variant", VARIANTS, ids=VARIANT_IDS)
