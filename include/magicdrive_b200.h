@@ -42,6 +42,12 @@ int mdb_device_ok(void);
  *                           + bias[n] + rowbias[img(pix), n] ) + residual[pix, n]
  *   epi_mode 1 (GEGLU): W/bias are packed per 256-column tile as [128 value | 128 gate] and
  *   out[pix, j] = value_j * gelu(gate_j) with n_out/2 output columns.
+ * Channel counts c0, c1 are multiples of 8.  The K loop runs over 64-channel blocks per filter tap; when c % 64 != 0 the
+ * last block of each tap is partial (channels past c read as zeros), so W is packed per tap at the width rounded up to 64:
+ *   W[n, tap*K64 + c] with K64 = 64*ceil(c0/64) + 64*ceil(c1/64), source 1 starting at column 64*ceil(c0/64), zeros in
+ *   the gaps.  For channel counts that are multiples of 64 this is the plain (tap, channel) layout.
+ * Filters are taps_h x taps_w with padding pad_h / pad_w (1x7, 7x1, 5x5, ...); the TMA im2col limits apply:
+ * -128 <= -pad and pad - (taps - 1) <= 127 per dimension, else MDB_ERR_UNSUPPORTED.
  * Replaces: nn.Conv2d 3x3/1x1 in ResnetBlock2D (diffusers/models/resnet.py:537,560,586), Downsample2D
  * (resnet.py:199), Upsample2D.conv (resnet.py:129), Transformer2DModel.proj_in/proj_out
  * (transformer_2d.py:149,205), Attention.to_q/to_k/to_v/to_out (attention_processor.py:141-156),
@@ -54,7 +60,7 @@ typedef struct {
   const void* a1;      /* optional second source (NULL if c1 == 0) */
   int c0, lda0, c1, lda1;
   int n_img, h_in, w_in;
-  const void* w;       /* bf16 [n_out, taps_h*taps_w*(c0+c1)] */
+  const void* w;       /* bf16 [n_out, taps_h*taps_w*K64] (K64 = c0+c1 rounded up per source to 64, see above) */
   int n_out;
   int taps_h, taps_w, stride, pad_h, pad_w;
   int h_out, w_out;
@@ -69,7 +75,10 @@ typedef struct {
   float out_scale;
   int epi_mode;         /* 0 linear, 1 GEGLU, 2 quick-GELU: out = y * sigmoid(1.702 y) on y = the linear epilogue's value
                          * (CLIP MLP fc1, transformers models/clip/modeling_clip.py CLIPMLP); never split-K, no residual,
-                         * rowbias, stats_out or fp32 output */
+                         * rowbias, stats_out or fp32 output; 3 ReLU: out = max(0, v) on v = the linear epilogue's value
+                         * (bias, out_scale), for a BatchNorm folded into W / bias followed by ReLU (torchvision Inception3
+                         * BasicConv2d); plain bf16 output only (no residual, rowbias, stats_out or fp32 output); split-K
+                         * applies it in the finalize pass.  ReLU launches run their own kernel instantiations. */
   void* workspace;      /* split-K scratch (may be NULL => no split-K) */
   size_t workspace_bytes;
   int force_block_n;    /* 0 = auto; test hook */
@@ -100,6 +109,26 @@ int mdb_gemm_conv_stats_parts(const mdb_gemm_desc* d);
 /* The planner's tiling for this descriptor, for profiling tools: plan[0..4] = block_n, M tiles, N tiles, K splits,
  * waves of the persistent grid. */
 int mdb_gemm_conv_plan(const mdb_gemm_desc* d, int* plan);
+
+/* ------------------------------------------------------------------------------------------------
+ * FID Inception helpers (magicdrive/misc/inception.py InceptionV3 with fid_inception_v3(), inception.py:129-163, 197-341).
+ * mdb_pool2d over NHWC bf16 [n, h, w, ldx] using the first c channels (c, ldx, ldo multiples of 8, 16-byte aligned
+ * pointers), writing into the first c columns of out [n*ho*wo, ldo] -- a column slice of a wider buffer, so the Inception
+ * blocks' torch.cat is never materialised:
+ *   mode 0: max over the k x k window at stride, padding ignored (F.max_pool2d / nn.MaxPool2d, inception.py:89,98,337);
+ *   mode 1: average over the window's in-image pixels (F.avg_pool2d count_include_pad=False, inception.py:241,269,302);
+ *   mode 2: global average of each image into fp32 out [n, ldo] (nn.AdaptiveAvgPool2d(1), inception.py:122);
+ *           k, stride, pad, ho, wo are ignored.
+ * mdb_fid_input: a [0, 1] image batch, fp32 or bf16, NCHW [n, 3, h, w] or (x_is_nhwc) NHWC [n, h, w, 3] -> bf16 NHWC
+ * [n, ho, wo, 8] with channels 3..7 zero (the K-padded A operand of Conv2d_1a_3x3 on mdb_gemm_conv, c0 = 8):
+ *   quantize: x = rint(255 x) / 255 clamped to [0, 1], the 8-bit levels a saved PNG holds (diffusers pil_utils.py:41);
+ *   bilinear resize to ho x wo with F.interpolate(align_corners=False) semantics, no antialias (inception.py:146-150)
+ *   (ho == h and wo == w is the identity); normalize: 2x - 1 (inception.py:152-153).
+ * ------------------------------------------------------------------------------------------------ */
+int mdb_pool2d(const void* x, int ldx, int n, int h, int w, int c, int mode, int k, int stride, int pad, void* out,
+               int ldo, int ho, int wo, void* stream);
+int mdb_fid_input(const void* x, int x_is_f32, int x_is_nhwc, int n, int h, int w, int quantize, int normalize, void* out,
+                  int ho, int wo, void* stream);
 
 /* Direct (CUDA-core) convolution for tiny channel counts: conv_in 4->320 (unet_2d_condition.py:231),
  * conv_out 320->4 (:503), BEV map encoder (magicdrive/networks/map_embedder.py:66-76).

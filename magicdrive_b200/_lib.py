@@ -71,6 +71,8 @@ SIGNATURES = {
     "mdb_prepare_boxes": (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "mdb_camera_param": (_i, [_vp, _vp, _i, _vp, _vp]),
     "mdb_cfg_unipc_step": (_i, [_vp, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _ll, _vp]),
+    "mdb_pool2d": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),
+    "mdb_fid_input": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _vp]),
 }
 
 

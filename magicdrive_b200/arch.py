@@ -477,3 +477,129 @@ def synthetic_state_dict(shapes, seed: int = 0, scale: float = 1.0):
     with ThreadPoolExecutor(max_workers=min(16, os.cpu_count() or 1)) as ex:
         sd = OrderedDict(ex.map(make, items))
     return sd
+
+
+# ------------------------------------------------------------------------------------------ FID InceptionV3
+# The FID variant of torchvision's Inception3 as magicdrive/misc/inception.py:197-221 (fid_inception_v3) assembles it:
+# num_classes=1008, aux_logits=False, Mixed_5b-5d = FIDInceptionA, Mixed_6b-6e = FIDInceptionC, Mixed_7b / 7c =
+# FIDInceptionE_1 / _2, Mixed_6a / 7a = torchvision's InceptionB / InceptionD.  Every BasicConv2d is a bias-free conv,
+# BatchNorm2d(eps=0.001) and ReLU (torchvision models/inception.py BasicConv2d).
+INCEPTION_BN_EPS = 1e-3
+INCEPTION_SIZE = 299
+INCEPTION_DIMS = (64, 192, 768, 2048)  # channels of the four output blocks (inception.py:24-29)
+
+
+@dataclass(frozen=True)
+class InceptionConv:
+    name: str  # torchvision module name (the pytorch-fid weights file's keys), e.g. "Mixed_6b.branch7x7_2"
+    cin: int
+    cout: int
+    kh: int
+    kw: int
+    stride: int = 1
+    ph: int = 0
+    pw: int = 0
+
+
+# (module, kind, in_channels, pool_features / channels_7x7) of InceptionV3 blocks 2 and 3 (inception.py:103-124)
+INCEPTION_MIXED = (
+    ("Mixed_5b", "A", 192, 32), ("Mixed_5c", "A", 256, 64), ("Mixed_5d", "A", 288, 64), ("Mixed_6a", "B", 288, 0),
+    ("Mixed_6b", "C", 768, 128), ("Mixed_6c", "C", 768, 160), ("Mixed_6d", "C", 768, 160), ("Mixed_6e", "C", 768, 192),
+    ("Mixed_7a", "D", 768, 0), ("Mixed_7b", "E1", 1280, 0), ("Mixed_7c", "E2", 2048, 0),
+)
+# torchvision module names of each InceptionV3 block's layers (inception.py:84-124); pools carry no parameters
+INCEPTION_BLOCKS = (
+    ("Conv2d_1a_3x3", "Conv2d_2a_3x3", "Conv2d_2b_3x3"),
+    ("Conv2d_3b_1x1", "Conv2d_4a_3x3"),
+    ("Mixed_5b", "Mixed_5c", "Mixed_5d", "Mixed_6a", "Mixed_6b", "Mixed_6c", "Mixed_6d", "Mixed_6e"),
+    ("Mixed_7a", "Mixed_7b", "Mixed_7c"),
+)
+
+
+def mixed_out_channels(kind: str, cin: int, arg: int) -> int:
+    return {"A": 224 + arg, "B": 384 + 96 + cin, "C": 768, "D": 320 + 192 + cin, "E1": 2048, "E2": 2048}[kind]
+
+
+def _mixed_convs(m: str, kind: str, cin: int, arg: int) -> List[InceptionConv]:
+    """Convolutions of one Mixed block in torchvision's registration order (models/inception.py InceptionA-E)."""
+    C = lambda s, ci, co, kh, kw, st=1, ph=0, pw=0: InceptionConv(f"{m}.{s}", ci, co, kh, kw, st, ph, pw)
+    if kind == "A":
+        return [C("branch1x1", cin, 64, 1, 1), C("branch5x5_1", cin, 48, 1, 1), C("branch5x5_2", 48, 64, 5, 5, 1, 2, 2),
+                C("branch3x3dbl_1", cin, 64, 1, 1), C("branch3x3dbl_2", 64, 96, 3, 3, 1, 1, 1),
+                C("branch3x3dbl_3", 96, 96, 3, 3, 1, 1, 1), C("branch_pool", cin, arg, 1, 1)]
+    if kind == "B":
+        return [C("branch3x3", cin, 384, 3, 3, 2), C("branch3x3dbl_1", cin, 64, 1, 1),
+                C("branch3x3dbl_2", 64, 96, 3, 3, 1, 1, 1), C("branch3x3dbl_3", 96, 96, 3, 3, 2)]
+    if kind == "C":
+        c7 = arg
+        return [C("branch1x1", cin, 192, 1, 1), C("branch7x7_1", cin, c7, 1, 1), C("branch7x7_2", c7, c7, 1, 7, 1, 0, 3),
+                C("branch7x7_3", c7, 192, 7, 1, 1, 3, 0), C("branch7x7dbl_1", cin, c7, 1, 1),
+                C("branch7x7dbl_2", c7, c7, 7, 1, 1, 3, 0), C("branch7x7dbl_3", c7, c7, 1, 7, 1, 0, 3),
+                C("branch7x7dbl_4", c7, c7, 7, 1, 1, 3, 0), C("branch7x7dbl_5", c7, 192, 1, 7, 1, 0, 3),
+                C("branch_pool", cin, 192, 1, 1)]
+    if kind == "D":
+        return [C("branch3x3_1", cin, 192, 1, 1), C("branch3x3_2", 192, 320, 3, 3, 2),
+                C("branch7x7x3_1", cin, 192, 1, 1), C("branch7x7x3_2", 192, 192, 1, 7, 1, 0, 3),
+                C("branch7x7x3_3", 192, 192, 7, 1, 1, 3, 0), C("branch7x7x3_4", 192, 192, 3, 3, 2)]
+    return [C("branch1x1", cin, 320, 1, 1), C("branch3x3_1", cin, 384, 1, 1), C("branch3x3_2a", 384, 384, 1, 3, 1, 0, 1),
+            C("branch3x3_2b", 384, 384, 3, 1, 1, 1, 0), C("branch3x3dbl_1", cin, 448, 1, 1),
+            C("branch3x3dbl_2", 448, 384, 3, 3, 1, 1, 1), C("branch3x3dbl_3a", 384, 384, 1, 3, 1, 0, 1),
+            C("branch3x3dbl_3b", 384, 384, 3, 1, 1, 1, 0), C("branch_pool", cin, 192, 1, 1)]
+
+
+def inception_convs(last_block: int = 3) -> "OrderedDict[str, Tuple[str, InceptionConv]]":
+    """torchvision name -> (InceptionV3 wrapper prefix `blocks.{i}.{j}[.branch]`, conv) for blocks 0..last_block."""
+    stem = {"Conv2d_1a_3x3": InceptionConv("Conv2d_1a_3x3", 3, 32, 3, 3, 2),
+            "Conv2d_2a_3x3": InceptionConv("Conv2d_2a_3x3", 32, 32, 3, 3),
+            "Conv2d_2b_3x3": InceptionConv("Conv2d_2b_3x3", 32, 64, 3, 3, 1, 1, 1),
+            "Conv2d_3b_1x1": InceptionConv("Conv2d_3b_1x1", 64, 80, 1, 1),
+            "Conv2d_4a_3x3": InceptionConv("Conv2d_4a_3x3", 80, 192, 3, 3)}
+    mixed = {m: (kind, cin, arg) for m, kind, cin, arg in INCEPTION_MIXED}
+    out = OrderedDict()
+    for i, mods in enumerate(INCEPTION_BLOCKS[: last_block + 1]):
+        for j, m in enumerate(mods):
+            if m in stem:
+                out[m] = (f"blocks.{i}.{j}", stem[m])
+            else:
+                for cv in _mixed_convs(m, *mixed[m]):
+                    out[cv.name] = (f"blocks.{i}.{j}.{cv.name.split('.', 1)[1]}", cv)
+    return out
+
+
+INCEPTION_BN_BUFFERS = ("running_mean", "running_var", "num_batches_tracked")
+
+
+def inception_param_shapes(last_block: int = 3) -> "OrderedDict[str, tuple]":
+    """State-dict keys and shapes of magicdrive/misc/inception.py InceptionV3 built with max(output_blocks) = last_block."""
+    sh = OrderedDict()
+    for prefix, cv in inception_convs(last_block).values():
+        sh[prefix + ".conv.weight"] = (cv.cout, cv.cin, cv.kh, cv.kw)
+        for s in ("weight", "bias", "running_mean", "running_var"):
+            sh[f"{prefix}.bn.{s}"] = (cv.cout,)
+        sh[prefix + ".bn.num_batches_tracked"] = ()
+    return sh
+
+
+def inception_synthetic_state_dict(last_block: int = 3, seed: int = 0):
+    """Seeded weights under the wrapper's names (Philox per tensor name, like arch.synthetic_state_dict) with sane
+    BatchNorm statistics: gains near 1, running_var in [0.5, 1.5], so the features are neither degenerate nor exploding."""
+    import zlib
+
+    import numpy as np
+    import torch
+    sd = OrderedDict()
+    for name, shape in inception_param_shapes(last_block).items():
+        rng = np.random.Generator(np.random.Philox(key=(seed << 32) + zlib.crc32(name.encode())))
+        if name.endswith("num_batches_tracked"):
+            sd[name] = torch.zeros((), dtype=torch.long)
+            continue
+        if name.endswith("conv.weight"):
+            a = rng.standard_normal(shape, dtype=np.float32) * np.float32(np.sqrt(2.0 / np.prod(shape[1:])))
+        elif name.endswith("bn.weight"):
+            a = 1.0 + 0.1 * rng.standard_normal(shape, dtype=np.float32)
+        elif name.endswith("running_var"):
+            a = rng.uniform(0.5, 1.5, shape).astype(np.float32)
+        else:  # bn.bias, running_mean
+            a = 0.1 * rng.standard_normal(shape, dtype=np.float32)
+        sd[name] = torch.from_numpy(np.ascontiguousarray(a.astype(np.float32)))
+    return sd

@@ -17,7 +17,7 @@ NVCC_FLAGS = [
     "-Xcompiler", "-fPIC", "--use_fast_math",
 ]
 # --use_fast_math is NOT applied to the files listed here (exact erf/sin/cos/exp paths that parity tests pin)
-PRECISE = {"capi_pointwise.cu", "capi_gemm.cu", "capi_inputprep.cu"}
+PRECISE = {"capi_pointwise.cu", "capi_gemm.cu", "capi_inputprep.cu", "capi_fid.cu"}
 
 
 def _sources():

@@ -82,10 +82,14 @@ int num_sms() {
   return sms;
 }
 
+// 64-wide K blocks per filter tap of a source with c channels: the last one is partial when c % 64 != 0 (the TMA
+// zero-fills the channels past c, and the weights hold zeros in the same K columns)
+inline int cblocks(int c) { return (c + kBlockK - 1) / kBlockK; }
+
 int validate(const mdb_gemm_desc* d) {
   if (!d || !d->a0 || !d->w || !d->out) return set_error(MDB_ERR_INVALID, "mdb_gemm_conv: null pointer");
-  if (d->c0 <= 0 || d->c0 % 64 || d->c1 < 0 || d->c1 % 64)
-    return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: channel counts must be multiples of 64 (c0=%d c1=%d)", d->c0,
+  if (d->c0 <= 0 || d->c0 % 8 || d->c1 < 0 || d->c1 % 8)
+    return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: channel counts must be multiples of 8 (c0=%d c1=%d)", d->c0,
                      d->c1);
   if (d->c1 > 0 && !d->a1) return set_error(MDB_ERR_INVALID, "mdb_gemm_conv: c1>0 but a1 is null");
   if (d->lda0 % 8 || (d->c1 > 0 && d->lda1 % 8) || d->ldo % 8 || (d->residual && d->ldr % 8))
@@ -105,7 +109,17 @@ int validate(const mdb_gemm_desc* d) {
   if (d->epi_mode == 2 && (d->residual || d->rowbias || d->out_is_f32 || d->stats_out))
     return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: quick-GELU epilogue needs a plain bf16 output "
                                           "(no residual, per-image shift or row statistics)");
-  if (d->epi_mode < 0 || d->epi_mode > 2) return set_error(MDB_ERR_INVALID, "mdb_gemm_conv: epi_mode must be 0, 1 or 2");
+  if (d->epi_mode == 3 && (d->residual || d->rowbias || d->out_is_f32 || d->stats_out))
+    return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: ReLU epilogue needs a plain bf16 output "
+                                          "(no residual, per-image shift or row statistics)");
+  if (d->epi_mode < 0 || d->epi_mode > 3)
+    return set_error(MDB_ERR_INVALID, "mdb_gemm_conv: epi_mode must be 0, 1, 2 or 3");
+  // im2col bounding-box corners of a 4-D map are signed 8-bit and the per-tap offsets unsigned 8-bit
+  const int corners[4] = {-d->pad_w, -d->pad_h, d->pad_w - (d->taps_w - 1), d->pad_h - (d->taps_h - 1)};
+  for (int i = 0; i < 4; ++i)
+    if (corners[i] < -128 || corners[i] > 127 || d->taps_h > 256 || d->taps_w > 256)
+      return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: filter %dx%d with padding %dx%d exceeds the TMA im2col limits",
+                       d->taps_h, d->taps_w, d->pad_h, d->pad_w);
   return MDB_OK;
 }
 
@@ -115,7 +129,7 @@ void plan_for(const mdb_gemm_desc* d, int ctas, bool allow_split, Plan* pl) {
   pl->m_tiles = m_tiles;
   pl->ctas = ctas;
   pl->m_groups = (m_tiles + ctas - 1) / ctas;
-  pl->kb_total = d->taps_h * d->taps_w * ((d->c0 + d->c1) / 64);
+  pl->kb_total = d->taps_h * d->taps_w * (cblocks(d->c0) + cblocks(d->c1));
   const int sms = num_sms();
   const int clusters = sms / ctas;
   int bn_choice = 0;
@@ -146,7 +160,7 @@ void plan_for(const mdb_gemm_desc* d, int ctas, bool allow_split, Plan* pl) {
     splits = 1;
   } else if (d->force_splits > 0) {
     splits = d->force_splits;
-  } else if (d->epi_mode == 0 && !d->ln_stats && !d->stats_out && d->workspace && ctas_total * 2 <= sms && pl->kb_total >= 16) {
+  } else if ((d->epi_mode == 0 || d->epi_mode == 3) && !d->ln_stats && !d->stats_out && d->workspace && ctas_total * 2 <= sms && pl->kb_total >= 16) {
     splits = (int)(sms / ctas_total);
     if (splits > pl->kb_total / 8) splits = pl->kb_total / 8;
     if (splits > 16) splits = 16;
@@ -155,7 +169,8 @@ void plan_for(const mdb_gemm_desc* d, int ctas, bool allow_split, Plan* pl) {
   if (splits > pl->kb_total) splits = pl->kb_total;
   if (splits > 1) {
     const size_t need = (size_t)splits * d->n_img * d->h_out * d->w_out * d->n_out * sizeof(float);
-    if (!d->workspace || d->workspace_bytes < need || d->epi_mode != 0 || d->ln_stats || d->stats_out) splits = 1;
+    const bool linear = d->epi_mode == 0 || d->epi_mode == 3;  // the finalize pass applies the linear epilogue (+ ReLU)
+    if (!d->workspace || d->workspace_bytes < need || !linear || d->ln_stats || d->stats_out) splits = 1;
   }
   pl->kb_per_split = (pl->kb_total + splits - 1) / splits;
   pl->splits = (pl->kb_total + pl->kb_per_split - 1) / pl->kb_per_split;  // no empty split
@@ -169,12 +184,13 @@ void make_plan(const mdb_gemm_desc* d, Plan* pl) {
   plan_for(d, 1, d->kernel_variant != 4, pl);
 }
 
-template <int BN, int CTAS>
+template <int BN, int CTAS, bool RELU>
 int launch(const CUtensorMap& tA0, const CUtensorMap& tA1, const CUtensorMap& tB, const GemmParams& gp, cudaStream_t st) {
   using Cfg = WgGemmCfg<BN, CTAS>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, CTAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, CTAS, RELU>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         Cfg::kSmemBytes);
     if (e != cudaSuccess) return set_error(MDB_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     attr_set = true;
   }
@@ -192,20 +208,21 @@ int launch(const CUtensorMap& tA0, const CUtensorMap& tA1, const CUtensorMap& tB
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   add_pdl_attr(cfg, attr, 1);
-  cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<BN, CTAS>, tA0, tA1, tB, gp);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<BN, CTAS, RELU>, tA0, tA1, tB, gp);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MDB_ERR_CUDA, "gemm_wgmma_kernel<%d,%d> launch: %s", BN, CTAS, cudaGetErrorString(e));
   return MDB_OK;
 }
 
-template <int CTAS>
+template <int CTAS, bool RELU = false>
 int launch_bn(int block_n, const CUtensorMap& tA0, const CUtensorMap& tA1, const CUtensorMap& tB, const GemmParams& gp,
               cudaStream_t st) {
+  if (!RELU && gp.epi_mode == EPI_RELU) return launch_bn<CTAS, true>(block_n, tA0, tA1, tB, gp, st);
   switch (block_n) {
-    case 256: return launch<256, CTAS>(tA0, tA1, tB, gp, st);
-    case 160: return launch<160, CTAS>(tA0, tA1, tB, gp, st);
-    case 128: return launch<128, CTAS>(tA0, tA1, tB, gp, st);
-    case 64: return launch<64, CTAS>(tA0, tA1, tB, gp, st);
+    case 256: return launch<256, CTAS, RELU>(tA0, tA1, tB, gp, st);
+    case 160: return launch<160, CTAS, RELU>(tA0, tA1, tB, gp, st);
+    case 128: return launch<128, CTAS, RELU>(tA0, tA1, tB, gp, st);
+    case 64: return launch<64, CTAS, RELU>(tA0, tA1, tB, gp, st);
     default: return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: unsupported block_n %d", block_n);
   }
 }
@@ -264,7 +281,7 @@ extern "C" int mdb_gemm_conv(const mdb_gemm_desc* d, void* stream) {
   } else {
     tA1 = tA0;
   }
-  const int ktot = d->taps_h * d->taps_w * (d->c0 + d->c1);
+  const int ktot = d->taps_h * d->taps_w * kBlockK * (cblocks(d->c0) + cblocks(d->c1));
   if (!make_w_map(&tB, d->w, d->n_out, ktot, pl.block_n / pl.ctas))
     return set_error(MDB_ERR_CUDA, "cuTensorMapEncodeTiled(W) failed (n=%d k=%d)", d->n_out, ktot);
 
@@ -272,12 +289,15 @@ extern "C" int mdb_gemm_conv(const mdb_gemm_desc* d, void* stream) {
   memset(&gp, 0, sizeof(gp));
   gp.n_img = d->n_img, gp.h_out = d->h_out, gp.w_out = d->w_out, gp.n_out = d->n_out;
   gp.taps_h = d->taps_h, gp.taps_w = d->taps_w, gp.stride = d->stride, gp.pad_h = d->pad_h, gp.pad_w = d->pad_w;
-  gp.cblocks0 = d->c0 / 64, gp.cblocks1 = d->c1 / 64;
+  gp.cblocks0 = cblocks(d->c0), gp.cblocks1 = cblocks(d->c1);
   gp.im2col = im2col;
   gp.m_tiles = pl.m_tiles, gp.n_tiles = pl.n_tiles, gp.splits = pl.splits;
   gp.m_groups = pl.m_groups;
   gp.kb_per_split = pl.kb_per_split;
-  gp.epi_mode = pl.splits > 1 ? EPI_PARTIAL_F32 : d->epi_mode == 2 ? EPI_QUICK_GELU : d->epi_mode;
+  gp.epi_mode = pl.splits > 1      ? EPI_PARTIAL_F32
+                : d->epi_mode == 2 ? EPI_QUICK_GELU
+                : d->epi_mode == 3 ? EPI_RELU
+                                   : d->epi_mode;
   gp.out_is_f32 = d->out_is_f32;
   gp.bias = d->bias, gp.rowbias = d->rowbias, gp.rowbias_ld = d->rowbias_ld;
   gp.residual = static_cast<const __nv_bfloat16*>(d->residual), gp.ldr = d->ldr;
@@ -294,10 +314,11 @@ extern "C" int mdb_gemm_conv(const mdb_gemm_desc* d, void* stream) {
     const long long total4 = pixels * d->n_out / 4;
     const int threads = 256;
     const int blocks = (int)((total4 + threads - 1) / threads);
-    cudaError_t e = launch_pdl(splitk_finalize_kernel, dim3(blocks), dim3(threads), 0, st,
-                               static_cast<const float*>(d->workspace), pl.splits, pixels, d->n_out, d->h_out * d->w_out,
-                               d->bias, d->rowbias, d->rowbias_ld, static_cast<const __nv_bfloat16*>(d->residual), d->ldr,
-                               d->out, d->ldo, d->out_is_f32, d->out_scale);
+    cudaError_t e = launch_pdl(d->epi_mode == 3 ? splitk_finalize_kernel<true> : splitk_finalize_kernel<false>, dim3(blocks),
+                               dim3(threads), 0, st, static_cast<const float*>(d->workspace), pl.splits, pixels, d->n_out,
+                               d->h_out * d->w_out, d->bias, d->rowbias, d->rowbias_ld,
+                               static_cast<const __nv_bfloat16*>(d->residual), d->ldr, d->out, d->ldo, d->out_is_f32,
+                               d->out_scale);
     if (e == cudaSuccess) e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(MDB_ERR_CUDA, "splitk_finalize launch: %s", cudaGetErrorString(e));
   }

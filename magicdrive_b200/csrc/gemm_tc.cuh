@@ -20,8 +20,8 @@
 
 namespace mdb {
 
-// EPI_QUICK_GELU is mdb_gemm_desc.epi_mode 2 (internal 2 is the split-K partial store)
-enum EpiMode : int { EPI_LINEAR = 0, EPI_GEGLU = 1, EPI_PARTIAL_F32 = 2, EPI_QUICK_GELU = 3 };
+// EPI_QUICK_GELU is mdb_gemm_desc.epi_mode 2 (internal 2 is the split-K partial store), EPI_RELU is epi_mode 3
+enum EpiMode : int { EPI_LINEAR = 0, EPI_GEGLU = 1, EPI_PARTIAL_F32 = 2, EPI_QUICK_GELU = 3, EPI_RELU = 4 };
 
 struct GemmParams {
   // output pixel grid
@@ -29,7 +29,7 @@ struct GemmParams {
   int n_out;  // GEMM N (for GEGLU: the packed 2x width)
   // filter
   int taps_h, taps_w, stride, pad_h, pad_w;
-  int cblocks0, cblocks1;  // 64-channel blocks of A source 0 / 1
+  int cblocks0, cblocks1;  // 64-channel blocks of A source 0 / 1 (the last one partial, zero-filled, if C % 64 != 0)
   int im2col;              // A maps: 1 = 4-D im2col (convolutions), 0 = 2-D [pixels, C] (1x1)
   int m_tiles, n_tiles, splits;  // tiles = m_tiles * n_tiles * splits (m fastest); m_tiles = ceil(pixels / 128)
   int m_groups;                  // ceil(m_tiles / CTAS): M tiles are walked in groups of one per CTA of a cluster
@@ -87,7 +87,8 @@ __device__ __forceinline__ float quick_gelu(float x) {
   return x * r;
 }
 
-// Deterministic split-K finalisation: sum the fp32 partials in split order, then the same linear epilogue.
+// Deterministic split-K finalisation: sum the fp32 partials in split order, then the same linear epilogue (+ ReLU).
+template <bool RELU = false>
 __global__ void splitk_finalize_kernel(const float* __restrict__ partial, int splits, long long pixels, int n_out,
                                        int hw_out, const float* __restrict__ bias, const float* __restrict__ rowbias,
                                        int rowbias_ld, const __nv_bfloat16* __restrict__ residual, int ldr,
@@ -113,6 +114,8 @@ __global__ void splitk_finalize_kernel(const float* __restrict__ partial, int sp
   for (int j = 0; j < 4; ++j) f[j] *= out_scale;
   if (residual)
     for (int j = 0; j < 4; ++j) f[j] += __bfloat162float(residual[pix * ldr + col + j]);
+  if constexpr (RELU)
+    for (int j = 0; j < 4; ++j) f[j] = fmaxf(f[j], 0.f);
   if (out_is_f32) {
     *reinterpret_cast<float4*>(static_cast<float*>(out) + pix * ldo + col) = make_float4(f[0], f[1], f[2], f[3]);
   } else {

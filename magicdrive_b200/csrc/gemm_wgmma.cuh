@@ -11,7 +11,8 @@
 //               the fp32 accumulator in registers, then the epilogue straight from those registers.
 // Epilogue (per element, fp32):  out = A_row * acc + ((bias_n + shift_img,n) * scale + B_row * colsum_n) [+ residual]
 //   with A_row = scale, B_row = 0, or -- LayerNorm folded into this GEMM -- A_row = rstd * scale, B_row = -mean * rstd * scale
-//   from the per-row partial sums the producer of A emitted.  GEGLU tiles hold [128 value | 128 gate] columns.  Split-K
+//   from the per-row partial sums the producer of A emitted; ReLU launches store max(0, out).  GEGLU tiles hold
+//   [128 value | 128 gate] columns.  Split-K
 //   tiles write fp32 partials instead (summed in split order by splitk_finalize_kernel).
 #pragma once
 #include "common_host.h"
@@ -40,7 +41,8 @@ struct WgGemmCfg {
 
 __device__ __forceinline__ float2 ldg_f2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
 
-template <int BLOCK_N, int CTAS>
+// RELU: the ReLU epilogue (EPI_RELU) is compiled only into its own instantiations, so the others are the plain kernel
+template <int BLOCK_N, int CTAS, bool RELU = false>
 __global__ void __launch_bounds__(WgGemmCfg<BLOCK_N, CTAS>::kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                   const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
@@ -253,6 +255,24 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
           const float v1 = fmaf(rowA[h], acc[4 * j + 2 * h + 1], fmaf(rowB[h], cs.y, b.y * scale));
           *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.out) + pix[h] * p.ldo + col) =
               pack_bf16(quick_gelu(v0), quick_gelu(v1));
+        }
+      }
+      continue;
+    }
+    if constexpr (RELU) {  // its own loop too: plain bf16 output, the linear epilogue below is untouched
+#pragma unroll
+      for (int j = 0; j < BLOCK_N / 8; ++j) {
+        const int col = n0 + 8 * j + 2 * q;
+        if (col >= p.n_out) continue;
+        const float2 b = p.bias ? ldg_f2(p.bias + col) : make_float2(0.f, 0.f);
+        const float2 cs = has_ln ? ldg_f2(p.ln_colsum + col) : make_float2(0.f, 0.f);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!ok[h]) continue;
+          const float v0 = fmaf(rowA[h], acc[4 * j + 2 * h], fmaf(rowB[h], cs.x, b.x * scale));
+          const float v1 = fmaf(rowA[h], acc[4 * j + 2 * h + 1], fmaf(rowB[h], cs.y, b.y * scale));
+          *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.out) + pix[h] * p.ldo + col) =
+              pack_bf16(fmaxf(v0, 0.f), fmaxf(v1, 0.f));
         }
       }
       continue;

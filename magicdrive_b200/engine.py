@@ -18,7 +18,7 @@ from typing import Dict, List, Optional
 import torch
 
 from . import arch, ops
-from .params import pack_conv_weight, pack_geglu
+from .params import pack_conv_weight, pack_conv_weight_k64, pack_geglu
 
 BF16, F32 = torch.bfloat16, torch.float32
 
@@ -774,3 +774,129 @@ class TextEncoderEngine:
         out = ops.layernorm(X, g, b, eps).view(n, L, C)
         pooled = out[torch.arange(n, device=out.device), ids.argmax(-1)]
         return out, pooled
+
+
+class InceptionEngine:
+    """The FID InceptionV3 (magicdrive/misc/inception.py:16-163 with fid_inception_v3(), :197-341) on the same
+    implicit-GEMM convolution: every BasicConv2d is one mdb_gemm_conv with its BatchNorm folded into bf16 weights and an
+    fp32 bias and ReLU in the epilogue; channel counts that are not multiples of 64 (3 -> 8, 32, 48, 80, 96, 160, 288, 448)
+    run on the kernel's partial K blocks.  Each branch of a Mixed block writes straight into its column slice of the
+    block's output (torch.cat is never materialised), and the pools write into theirs.  `sd` uses the InceptionV3
+    wrapper's names (arch.inception_param_shapes)."""
+
+    def __init__(self, sd, device, last_block: int = 3):
+        self.device, self.last_block = device, last_block
+        self.W = _Weights(sd, device)
+        self.convs = arch.inception_convs(last_block)
+
+    def _folded(self, name):
+        """BatchNorm(eps=1e-3) folded into the conv: W' = W * g / sqrt(v + eps) (bf16, K64-packed), b' = beta - m * that."""
+        W = self.W
+        if name + ".w" not in W.t:
+            p, cv = self.convs[name]
+            w = W.raw(p + ".conv.weight").float()
+            g, b = W.raw(p + ".bn.weight").float(), W.raw(p + ".bn.bias").float()
+            m, v = W.raw(p + ".bn.running_mean").float(), W.raw(p + ".bn.running_var").float()
+            s = g / torch.sqrt(v + arch.INCEPTION_BN_EPS)
+            w = w * s[:, None, None, None]
+            if cv.cin % 8:  # the RGB input is padded to 8 channels (mdb_fid_input)
+                w = torch.cat([w, w.new_zeros((w.shape[0], 8 - cv.cin % 8, cv.kh, cv.kw))], 1)
+            W.t[name + ".w"], W.t[name + ".b"] = pack_conv_weight_k64(w, dtype=W.fold_dtype), _f32(b - m * s)
+        return W.t[name + ".w"], W.t[name + ".b"]
+
+    def conv(self, name: str, x: FMap, out: Optional[torch.Tensor] = None, col: int = 0) -> FMap:
+        """BasicConv2d `name` on x; with `out`, the result goes to columns [col, col + cout) of out."""
+        cv = self.convs[name][1]
+        w, b = self._folded(name)
+        ho = (x.h + 2 * cv.ph - cv.kh) // cv.stride + 1
+        wo = (x.w + 2 * cv.pw - cv.kw) // cv.stride + 1
+        dst = None if out is None else out[:, col: col + cv.cout]
+        y = ops.gemm_conv(x.data, w, n_img=x.n, h_in=x.h, w_in=x.w, c0=x.c, lda0=x.data.stride(0), n_out=cv.cout,
+                          taps_h=cv.kh, taps_w=cv.kw, stride=cv.stride, pad_h=cv.ph, pad_w=cv.pw, bias=b, relu=True,
+                          out=dst)
+        return FMap(y if out is None else out, x.n, ho, wo, cv.cout if out is None else out.shape[1])
+
+    def _pool(self, x: FMap, mode, k, stride, pad, out=None, col=0) -> FMap:
+        ho, wo = (x.h + 2 * pad - k) // stride + 1, (x.w + 2 * pad - k) // stride + 1
+        dst = None if out is None else out[:, col: col + x.c]
+        y = ops.pool2d(x.data, n=x.n, h=x.h, w=x.w, c=x.c, ldx=x.data.stride(0), mode=mode, k=k, stride=stride, pad=pad,
+                       out=dst)
+        return FMap(y if out is None else out, x.n, ho, wo, x.c if out is None else out.shape[1])
+
+    def _buffer(self, x: FMap, h, w, c):
+        return torch.empty((x.n * h * w, c), dtype=x.data.dtype, device=x.data.device)
+
+    def mixed(self, m: str, kind: str, x: FMap) -> FMap:
+        """One Mixed block (torchvision InceptionA-E forward with the inception.py:224-341 patches)."""
+        c = self.conv
+        ho, wo = ((x.h - 3) // 2 + 1, (x.w - 3) // 2 + 1) if kind in ("B", "D") else (x.h, x.w)  # stride-2 reductions
+        if kind == "A":  # FIDInceptionA: 64 | 64 | 96 | pool_features
+            cout = self.convs[m + ".branch_pool"][1].cout + 224
+            out = self._buffer(x, x.h, x.w, cout)
+            c(m + ".branch1x1", x, out, 0)
+            c(m + ".branch5x5_2", c(m + ".branch5x5_1", x), out, 64)
+            c(m + ".branch3x3dbl_3", c(m + ".branch3x3dbl_2", c(m + ".branch3x3dbl_1", x)), out, 128)
+            c(m + ".branch_pool", self._pool(x, ops.POOL_AVG, 3, 1, 1), out, 224)
+        elif kind == "B":  # InceptionB: 384 | 96 | max pool (in)
+            out = self._buffer(x, ho, wo, 480 + x.c)
+            c(m + ".branch3x3", x, out, 0)
+            c(m + ".branch3x3dbl_3", c(m + ".branch3x3dbl_2", c(m + ".branch3x3dbl_1", x)), out, 384)
+            self._pool(x, ops.POOL_MAX, 3, 2, 0, out, 480)
+        elif kind == "C":  # FIDInceptionC: 192 | 192 | 192 | 192
+            out = self._buffer(x, x.h, x.w, 768)
+            c(m + ".branch1x1", x, out, 0)
+            c(m + ".branch7x7_3", c(m + ".branch7x7_2", c(m + ".branch7x7_1", x)), out, 192)
+            t = c(m + ".branch7x7dbl_1", x)
+            for i in (2, 3, 4):
+                t = c(f"{m}.branch7x7dbl_{i}", t)
+            c(m + ".branch7x7dbl_5", t, out, 384)
+            c(m + ".branch_pool", self._pool(x, ops.POOL_AVG, 3, 1, 1), out, 576)
+        elif kind == "D":  # InceptionD: 320 | 192 | max pool (in)
+            out = self._buffer(x, ho, wo, 512 + x.c)
+            c(m + ".branch3x3_2", c(m + ".branch3x3_1", x), out, 0)
+            t = c(m + ".branch7x7x3_3", c(m + ".branch7x7x3_2", c(m + ".branch7x7x3_1", x)))
+            c(m + ".branch7x7x3_4", t, out, 320)
+            self._pool(x, ops.POOL_MAX, 3, 2, 0, out, 512)
+        else:  # FIDInceptionE_1 / _2: 320 | 384 384 | 384 384 | 192; E_2 max-pools its pool branch (inception.py:333-337)
+            out = self._buffer(x, x.h, x.w, 2048)
+            c(m + ".branch1x1", x, out, 0)
+            t = c(m + ".branch3x3_1", x)
+            c(m + ".branch3x3_2a", t, out, 320)
+            c(m + ".branch3x3_2b", t, out, 704)
+            t = c(m + ".branch3x3dbl_2", c(m + ".branch3x3dbl_1", x))
+            c(m + ".branch3x3dbl_3a", t, out, 1088)
+            c(m + ".branch3x3dbl_3b", t, out, 1472)
+            c(m + ".branch_pool", self._pool(x, ops.POOL_AVG if kind == "E1" else ops.POOL_MAX, 3, 1, 1), out, 1856)
+        return FMap(out, x.n, ho, wo, out.shape[1])
+
+    def forward(self, images: torch.Tensor, *, nhwc: bool, quantize: bool, resize: bool, normalize: bool,
+                output_blocks=(3,)) -> List[torch.Tensor]:
+        """images: [0, 1] batch, NCHW (n, 3, h, w) or with nhwc (n, h, w, 3), fp32 or bf16, on the device.  Returns the
+        requested blocks as NCHW fp32 tensors in ascending block order (inception.py:129-163)."""
+        n = images.shape[0]
+        h, w = (images.shape[1], images.shape[2]) if nhwc else (images.shape[2], images.shape[3])
+        size = (arch.INCEPTION_SIZE, arch.INCEPTION_SIZE) if resize else (h, w)
+        x = FMap(ops.fid_input(images, nhwc=nhwc, quantize=quantize, normalize=normalize, size=size), n, *size, 8)
+        last = max(output_blocks)
+        outs = []
+        for i in range(last + 1):
+            if i == 0:
+                for m in arch.INCEPTION_BLOCKS[0]:
+                    x = self.conv(m, x)
+                x = self._pool(x, ops.POOL_MAX, 3, 2, 0)
+            elif i == 1:
+                for m in arch.INCEPTION_BLOCKS[1]:
+                    x = self.conv(m, x)
+                x = self._pool(x, ops.POOL_MAX, 3, 2, 0)
+            elif i == 2:
+                for m, kind, _, _ in arch.INCEPTION_MIXED[:8]:
+                    x = self.mixed(m, kind, x)
+            else:
+                for m, kind, _, _ in arch.INCEPTION_MIXED[8:]:
+                    x = self.mixed(m, kind, x)
+            if i in output_blocks:
+                if i == 3:
+                    outs.append(ops.pool2d(x.data, n=x.n, h=x.h, w=x.w, c=x.c, mode=ops.POOL_GLOBAL_AVG).view(n, x.c, 1, 1))
+                else:
+                    outs.append(ops.nhwc_to_nchw(x.data, x.n, x.c, x.h, x.w))
+        return outs

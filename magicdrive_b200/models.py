@@ -18,7 +18,7 @@ import torch
 import torch.nn as nn
 
 from . import arch, ops
-from .engine import ControlNetEngine, TextEncoderEngine, UNetEngine, VaeDecoderEngine
+from .engine import ControlNetEngine, InceptionEngine, TextEncoderEngine, UNetEngine, VaeDecoderEngine
 
 BF16, F32 = torch.bfloat16, torch.float32
 
@@ -613,3 +613,119 @@ class CLIPTextModel(_B200Module):
         if not return_dict:
             return (hidden, pooled)
         return CLIPTextModelOutput(hidden, pooled)
+
+
+class InceptionV3(nn.Module):
+    """Drop-in for magicdrive.misc.inception.InceptionV3 (pytorch-fid's FID Inception, inception.py:16-163): same
+    constructor kwargs, DEFAULT_BLOCK_INDEX / BLOCK_INDEX_BY_DIM, parameter names (`blocks.{i}.{j}...`) and forward(inp)
+    -> list of NCHW fp32 block outputs.  The arithmetic runs in engine.InceptionEngine on the sm_90a kernels, one CUDA
+    graph per input shape.  Nothing is downloaded: the module is built empty and the caller loads the weights
+    (`from_pretrained(path)` for the pytorch-fid `.pth`, or load_state_dict with either naming scheme).  Only the FID
+    variant exists and there is no backward."""
+
+    DEFAULT_BLOCK_INDEX = 3
+    BLOCK_INDEX_BY_DIM = {64: 0, 192: 1, 768: 2, 2048: 3}
+
+    def __init__(self, output_blocks=(DEFAULT_BLOCK_INDEX,), resize_input=True, normalize_input=True,
+                 requires_grad=False, use_fid_inception=True):
+        super().__init__()
+        if not use_fid_inception:
+            raise ValueError("only the FID Inception (use_fid_inception=True) is implemented")
+        if requires_grad:
+            raise ValueError("InceptionV3 here is inference-only: requires_grad=True is not supported")
+        self.resize_input, self.normalize_input = resize_input, normalize_input
+        self.output_blocks = sorted(output_blocks)
+        self.last_needed_block = max(output_blocks)
+        assert self.last_needed_block <= 3, "Last possible output block index is 3"
+        for key, shape in arch.inception_param_shapes(self.last_needed_block).items():
+            parts = key.split(".")
+            mod = self
+            for name in parts[:-1]:
+                if name not in mod._modules:
+                    mod.add_module(name, nn.Module())
+                mod = mod._modules[name]
+            if parts[-1] == "num_batches_tracked":
+                mod.register_buffer(parts[-1], torch.zeros(shape, dtype=torch.long))
+            elif parts[-1] in arch.INCEPTION_BN_BUFFERS:
+                mod.register_buffer(parts[-1], torch.empty(shape, dtype=F32))
+            else:
+                mod.register_parameter(parts[-1], nn.Parameter(torch.empty(shape, dtype=F32), requires_grad=False))
+        self._engine = None
+        self._graphs = {}
+
+    use_cuda_graph = True
+
+    @property
+    def device(self):
+        return next(self.parameters()).device
+
+    def load_state_dict(self, state_dict, strict=True, **kw):
+        """Accepts the reference wrapper's names and the pytorch-fid weights file's (torchvision Inception3 names such as
+        `Mixed_5b.branch1x1.bn.running_var`); `fc.*` and `num_batches_tracked` are ignored."""
+        tv = {name: prefix for name, (prefix, _) in arch.inception_convs(self.last_needed_block).items()}
+        all_tv = {m for b in arch.INCEPTION_BLOCKS for m in b}
+        sd = {}
+        for k, v in state_dict.items():
+            if k.startswith("fc.") or k.endswith("num_batches_tracked"):
+                continue
+            layer = k.rsplit(".", 2)[0]  # "<torchvision layer>.conv|bn.<tensor>"
+            if layer in tv:
+                k = tv[layer] + k[len(layer):]
+            elif layer.split(".")[0] in all_tv:
+                continue  # a layer of a block this module does not build (smaller output_blocks)
+            sd[k] = v
+        sd.update((k, v) for k, v in self.state_dict().items() if k.endswith("num_batches_tracked"))
+        r = super().load_state_dict(sd, strict=strict, **kw)
+        self._engine, self._graphs = None, {}
+        return r
+
+    def _apply(self, fn, *a, **k):
+        r = super()._apply(fn, *a, **k)
+        self._engine, self._graphs = None, {}
+        return r
+
+    @classmethod
+    def from_pretrained(cls, path, output_blocks=(DEFAULT_BLOCK_INDEX,), **kwargs):
+        """Build the module and load the pytorch-fid weights file (pt_inception-2015-12-05-6726825d.pth) from a local path."""
+        model = cls(output_blocks, **kwargs)
+        model.load_state_dict(torch.load(path, map_location="cpu", weights_only=True))
+        return model
+
+    def engine(self) -> InceptionEngine:
+        dev = self.device
+        if dev.type != "cuda":
+            raise ops._lib.MdbError(f"InceptionV3 runs only on a CUDA (sm_90a) device; parameters are on {dev}")
+        if self._engine is None:
+            self._engine = InceptionEngine(dict(self.state_dict()), dev, self.last_needed_block)
+        return self._engine
+
+    @torch.no_grad()
+    def features(self, images: torch.Tensor, nhwc: bool = False, quantize: bool = False) -> List[torch.Tensor]:
+        """The forward pass on a [0, 1] batch, NCHW (n, 3, h, w) or with nhwc (n, h, w, 3), optionally rounded to the 8-bit
+        levels a saved PNG holds first.  One CUDA graph per (shape, dtype, layout, rounding)."""
+        eng = self.engine()
+        images = images.to(self.device)
+        if images.dtype not in (F32, BF16):
+            images = images.float()
+        run = lambda x: eng.forward(x, nhwc=nhwc, quantize=quantize, resize=self.resize_input,
+                                    normalize=self.normalize_input, output_blocks=tuple(self.output_blocks))
+        if not self.use_cuda_graph:
+            return run(images.contiguous())
+        key = (tuple(images.shape), images.dtype, nhwc, quantize)
+        g = self._graphs.get(key)
+        if g is None:
+            xin = images.contiguous().clone()
+            run(xin)  # eager once: sizes the split-K scratch and packs the weights
+            torch.cuda.synchronize()
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                outs = run(xin)
+            g = self._graphs[key] = (graph, xin, outs)
+        graph, xin, outs = g
+        xin.copy_(images)
+        graph.replay()
+        return [o.clone() for o in outs]
+
+    def forward(self, inp: torch.Tensor) -> List[torch.Tensor]:
+        """inp: (N, 3, H, W) in [0, 1] -> the selected blocks' outputs, NCHW fp32, ascending block index."""
+        return self.features(inp)

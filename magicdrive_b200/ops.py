@@ -126,18 +126,26 @@ def gemm_conv(a0: torch.Tensor, w: torch.Tensor, *, n_img: int, h_in: int, w_in:
               ldo: Optional[int] = None, out_f32: bool = False, out_scale: float = 1.0, geglu: bool = False,
               force_block_n: int = 0, force_splits: int = 0, allow_split_k: bool = True, kernel_variant: int = 0,
               ln: Optional["RowStats"] = None, ln_colsum: Optional[torch.Tensor] = None, ln_eps: float = 1e-5,
-              emit_stats: bool = False, quick_gelu: bool = False):
+              emit_stats: bool = False, quick_gelu: bool = False, relu: bool = False, taps_h: Optional[int] = None,
+              taps_w: Optional[int] = None, pad_h: Optional[int] = None, pad_w: Optional[int] = None):
     """wgmma GEMM / implicit-GEMM conv (mdb_gemm_conv).  `a0` (and `a1`) are NHWC bf16 buffers whose pixel
-    stride is lda* elements; `w` is bf16 [n_out, taps*taps*(c0+c1)].
+    stride is lda* elements; `w` is bf16 [n_out, taps_h*taps_w*K64] with K64 = c0+c1, each rounded up to 64
+    (params.pack_conv_weight_k64; the plain (tap, channel) layout when c0 and c1 are multiples of 64).
+    `taps` / `pad` give a square filter; taps_h, taps_w, pad_h, pad_w override them per dimension (1x7, 7x1, ...).
+    relu: out = max(0, linear epilogue value) (a BatchNorm folded into w / bias, then ReLU).
     ln / ln_colsum: fold a LayerNorm of the rows of `a0` into this GEMM (`ln` = the RowStats the producer of `a0`
     emitted, `w` pre-multiplied by gamma, `bias` = beta-term + bias).  emit_stats: also return the RowStats of the
     output rows -> (out, RowStats).  quick_gelu: out = y * sigmoid(1.702 y) (CLIP's MLP activation)."""
     global _launches
     _need_cuda(a0, w)
+    th = taps if taps_h is None else taps_h
+    tw = taps if taps_w is None else taps_w
+    ph = pad if pad_h is None else pad_h
+    pw = pad if pad_w is None else pad_w
     if h_out is None:
-        h_out = (h_in + 2 * pad - taps) // stride + 1
+        h_out = (h_in + 2 * ph - th) // stride + 1
     if w_out is None:
-        w_out = (w_in + 2 * pad - taps) // stride + 1
+        w_out = (w_in + 2 * pw - tw) // stride + 1
     pixels = n_img * h_out * w_out
     width = n_out // 2 if geglu else n_out
     if out is None:
@@ -150,15 +158,15 @@ def gemm_conv(a0: torch.Tensor, w: torch.Tensor, *, n_img: int, h_in: int, w_in:
     d.c0, d.lda0, d.c1, d.lda1 = c0, lda0, c1, lda1
     d.n_img, d.h_in, d.w_in = n_img, h_in, w_in
     d.w, d.n_out = _ptr(w), n_out
-    d.taps_h = d.taps_w = taps
-    d.stride, d.pad_h, d.pad_w = stride, pad, pad
+    d.taps_h, d.taps_w = th, tw
+    d.stride, d.pad_h, d.pad_w = stride, ph, pw
     d.h_out, d.w_out = h_out, w_out
     d.bias = _ptr(bias)
     d.rowbias = _ptr(rowbias)
     d.rowbias_ld = (rowbias.stride(0) if rowbias.shape[0] > 1 else 0) if rowbias is not None else 0  # 1 row = shared by all images
     d.residual, d.ldr = _ptr(residual), ldr
     d.out, d.ldo, d.out_is_f32, d.out_scale = _ptr(out), ldo, int(out_f32), float(out_scale)
-    d.epi_mode = 1 if geglu else 2 if quick_gelu else 0
+    d.epi_mode = 1 if geglu else 2 if quick_gelu else 3 if relu else 0
     if allow_split_k and not geglu and not quick_gelu:
         ws = workspace(64 << 20, a0.device)
         d.workspace, d.workspace_bytes = ws.data_ptr(), ws.numel()
@@ -182,9 +190,9 @@ def gemm_conv(a0: torch.Tensor, w: torch.Tensor, *, n_img: int, h_in: int, w_in:
     if e0 is not None:
         plan = (C.c_int * 5)()
         check(L.mdb_gemm_conv_plan(C.byref(d), plan), "mdb_gemm_conv_plan")
-        _prof_end("gemm_conv", 2.0 * pixels * n_out * taps * taps * (c0 + c1), e0,
-                  f"M={pixels} N={n_out} K={taps * taps * (c0 + c1)} img={n_img}x{h_out}x{w_out} taps={taps} s={stride} "
-                  f"geglu={int(geglu)} qgelu={int(quick_gelu)} res={int(residual is not None)} | BN={plan[0]} tiles={plan[1]}x{plan[2]}x{plan[3]} "
+        _prof_end("gemm_conv", 2.0 * pixels * n_out * th * tw * (c0 + c1), e0,
+                  f"M={pixels} N={n_out} K={th * tw * (c0 + c1)} img={n_img}x{h_out}x{w_out} taps={th}x{tw} s={stride} "
+                  f"geglu={int(geglu)} qgelu={int(quick_gelu)} relu={int(relu)} res={int(residual is not None)} | BN={plan[0]} tiles={plan[1]}x{plan[2]}x{plan[3]} "
                   f"waves={plan[4]}")
     _launches += L.mdb_gemm_conv_launches(C.byref(d))
     return (out, stats) if emit_stats else out
@@ -375,6 +383,51 @@ def adaptive_avgpool(x, n, h, w, c, ho, wo, silu=False):
     assert x.dtype == F32 and x.is_contiguous()
     out = torch.empty((n, ho, wo, c), dtype=F32, device=x.device)
     check(_lib.lib().mdb_adaptive_avgpool(_ptr(x), n, h, w, c, _ptr(out), ho, wo, int(silu), _stream()), "mdb_adaptive_avgpool")
+    _launches += 1
+    return out
+
+
+POOL_MAX, POOL_AVG, POOL_GLOBAL_AVG = 0, 1, 2
+
+
+def pool2d(x, *, n, h, w, c, mode, k=3, stride=1, pad=0, ldx=None, out=None, ldo=None):
+    """mdb_pool2d over NHWC bf16 [n*h*w, ldx] (first c channels).  POOL_MAX: k x k max at stride, padding ignored;
+    POOL_AVG: average over the window's in-image pixels (count_include_pad=False); both write bf16 [n*ho*wo, ldo]
+    (a column slice of `out` when ldo > c).  POOL_GLOBAL_AVG: fp32 [n, ldo] per-image means."""
+    global _launches
+    _need_cuda(x)
+    ldx = c if ldx is None else ldx
+    if mode == POOL_GLOBAL_AVG:
+        ho = wo = 1
+        if out is None:
+            out, ldo = torch.empty((n, c), dtype=F32, device=x.device), c
+    else:
+        ho, wo = (h + 2 * pad - k) // stride + 1, (w + 2 * pad - k) // stride + 1
+        if out is None:
+            out, ldo = torch.empty((n * ho * wo, c), dtype=BF16, device=x.device), c
+    if ldo is None:
+        ldo = out.stride(0)
+    check(_lib.lib().mdb_pool2d(_ptr(x), ldx, n, h, w, c, mode, k, stride, pad, _ptr(out), ldo, ho, wo, _stream()),
+          "mdb_pool2d")
+    _launches += 1
+    return out
+
+
+def fid_input(x, *, nhwc: bool, quantize: bool, normalize: bool, size=None):
+    """mdb_fid_input: a [0, 1] image batch (NCHW [n, 3, h, w], or NHWC [n, h, w, 3] with nhwc=True; fp32 or bf16) ->
+    bf16 [n*ho*wo, 8] (channels 3..7 zero), optionally rounded to 8-bit levels, bilinearly resized to size = (ho, wo)
+    and mapped to 2x - 1."""
+    global _launches
+    _need_cuda(x)
+    x = x.contiguous()
+    if x.dtype not in (F32, BF16):
+        x = x.float()
+    n, h, w = (x.shape[0], x.shape[1], x.shape[2]) if nhwc else (x.shape[0], x.shape[2], x.shape[3])
+    assert (x.shape[3] if nhwc else x.shape[1]) == 3
+    ho, wo = (h, w) if size is None else size
+    out = torch.empty((n * ho * wo, 8), dtype=BF16, device=x.device)
+    check(_lib.lib().mdb_fid_input(_ptr(x), int(x.dtype == F32), int(nhwc), n, h, w, int(quantize), int(normalize), _ptr(out),
+                                   ho, wo, _stream()), "mdb_fid_input")
     _launches += 1
     return out
 
