@@ -47,7 +47,11 @@ int mdb_device_ok(void);
  *   W[n, tap*K64 + c] with K64 = 64*ceil(c0/64) + 64*ceil(c1/64), source 1 starting at column 64*ceil(c0/64), zeros in
  *   the gaps.  For channel counts that are multiples of 64 this is the plain (tap, channel) layout.
  * Filters are taps_h x taps_w with padding pad_h / pad_w (1x7, 7x1, 5x5, ...); the TMA im2col limits apply:
- * -128 <= -pad and pad - (taps - 1) <= 127 per dimension, else MDB_ERR_UNSUPPORTED.
+ * -128 <= -pad and pad + pad_end - (taps - 1) <= 127 per dimension, else MDB_ERR_UNSUPPORTED.
+ * pad_h_end / pad_w_end add zero rows below and zero columns right of the image on top of pad_h / pad_w (0 = symmetric
+ * padding), so h_out = (h_in + pad_h + pad_h_end - taps_h) / stride + 1: Downsample2D(padding=0) of the VAE encoder,
+ * F.pad(x, (0, 1, 0, 1)) then a 3x3 stride-2 conv (diffusers/models/resnet.py:199,215-217), is pad 0 with end pad 1.
+ * Negative end pads are MDB_ERR_INVALID.
  * Replaces: nn.Conv2d 3x3/1x1 in ResnetBlock2D (diffusers/models/resnet.py:537,560,586), Downsample2D
  * (resnet.py:199), Upsample2D.conv (resnet.py:129), Transformer2DModel.proj_in/proj_out
  * (transformer_2d.py:149,205), Attention.to_q/to_k/to_v/to_out (attention_processor.py:141-156),
@@ -98,6 +102,7 @@ typedef struct {
    * row (after bias / residual) over the columns of one N tile per slot, taken from the stored values (bf16-rounded for
    * bf16 outputs), or NULL. */
   float* stats_out;
+  int pad_h_end, pad_w_end;  /* extra zero rows below / columns right of the image (see above); 0 = symmetric padding */
 } mdb_gemm_desc;
 
 int mdb_gemm_conv(const mdb_gemm_desc* d, void* stream);

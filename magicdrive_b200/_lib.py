@@ -31,6 +31,7 @@ class GemmDesc(C.Structure):
         ("force_block_n", C.c_int), ("force_splits", C.c_int), ("kernel_variant", C.c_int),
         ("ln_stats", C.c_void_p), ("ln_parts", C.c_int), ("ln_eps", C.c_float), ("ln_colsum", C.c_void_p),
         ("stats_out", C.c_void_p),
+        ("pad_h_end", C.c_int), ("pad_w_end", C.c_int),
     ]
 
 

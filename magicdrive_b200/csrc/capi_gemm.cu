@@ -17,8 +17,8 @@ using namespace mdb;
 namespace {
 
 // A operand of a convolution: 4-D (C, W, H, N) im2col map, innermost first; pixel stride = ld elements.  The bounding box
-// of filter-tap-(0, 0) positions runs from -pad to (extent - 1 + pad - (taps - 1)) in each spatial dimension, walked with
-// the stride: exactly h_out x w_out positions per image.
+// of filter-tap-(0, 0) positions runs from -pad to (extent - 1 + pad + pad_end - (taps - 1)) in each spatial dimension,
+// walked with the stride: exactly h_out x w_out positions per image.
 bool make_im2col_map(CUtensorMap* m, const void* ptr, int c, int ld, const mdb_gemm_desc* d) {
   EncodeIm2colFn enc = get_encode_im2col();
   if (!enc) return false;
@@ -26,7 +26,7 @@ bool make_im2col_map(CUtensorMap* m, const void* ptr, int c, int ld, const mdb_g
   cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
   cuuint64_t strides[3] = {(cuuint64_t)ld * 2, (cuuint64_t)w * ld * 2, (cuuint64_t)h * w * ld * 2};
   int lower[2] = {-d->pad_w, -d->pad_h};
-  int upper[2] = {d->pad_w - (d->taps_w - 1), d->pad_h - (d->taps_h - 1)};
+  int upper[2] = {d->pad_w + d->pad_w_end - (d->taps_w - 1), d->pad_h + d->pad_h_end - (d->taps_h - 1)};
   cuuint32_t estr[4] = {1u, (cuuint32_t)d->stride, (cuuint32_t)d->stride, 1u};
   CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, lower, upper, 64u,
                    (cuuint32_t)kBlockM, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
@@ -114,12 +114,17 @@ int validate(const mdb_gemm_desc* d) {
                                           "(no residual, per-image shift or row statistics)");
   if (d->epi_mode < 0 || d->epi_mode > 3)
     return set_error(MDB_ERR_INVALID, "mdb_gemm_conv: epi_mode must be 0, 1, 2 or 3");
+  if (d->pad_h_end < 0 || d->pad_w_end < 0)
+    return set_error(MDB_ERR_INVALID, "mdb_gemm_conv: end padding must not be negative (pad_h_end=%d pad_w_end=%d)",
+                     d->pad_h_end, d->pad_w_end);
   // im2col bounding-box corners of a 4-D map are signed 8-bit and the per-tap offsets unsigned 8-bit
-  const int corners[4] = {-d->pad_w, -d->pad_h, d->pad_w - (d->taps_w - 1), d->pad_h - (d->taps_h - 1)};
+  const int corners[4] = {-d->pad_w, -d->pad_h, d->pad_w + d->pad_w_end - (d->taps_w - 1),
+                          d->pad_h + d->pad_h_end - (d->taps_h - 1)};
   for (int i = 0; i < 4; ++i)
     if (corners[i] < -128 || corners[i] > 127 || d->taps_h > 256 || d->taps_w > 256)
-      return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: filter %dx%d with padding %dx%d exceeds the TMA im2col limits",
-                       d->taps_h, d->taps_w, d->pad_h, d->pad_w);
+      return set_error(MDB_ERR_UNSUPPORTED,
+                       "mdb_gemm_conv: filter %dx%d with padding %dx%d (end %dx%d) exceeds the TMA im2col limits",
+                       d->taps_h, d->taps_w, d->pad_h, d->pad_w, d->pad_h_end, d->pad_w_end);
   return MDB_OK;
 }
 
@@ -268,8 +273,8 @@ extern "C" int mdb_gemm_conv(const mdb_gemm_desc* d, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 
   // output pixel p reads input pixel p unless the filter, stride, padding or output size say otherwise
-  const bool im2col = d->taps_h != 1 || d->taps_w != 1 || d->stride != 1 || d->pad_h || d->pad_w ||
-                      d->h_in != d->h_out || d->w_in != d->w_out;
+  const bool im2col = d->taps_h != 1 || d->taps_w != 1 || d->stride != 1 || d->pad_h || d->pad_w || d->pad_h_end ||
+                      d->pad_w_end || d->h_in != d->h_out || d->w_in != d->w_out;
   CUtensorMap tA0, tA1, tB;
   if (!make_act_map(&tA0, d->a0, d->c0, d->lda0, d, im2col))
     return set_error(MDB_ERR_CUDA, "cuTensorMapEncode%s(A0) failed (c=%d ld=%d n=%d h=%d w=%d taps=%dx%d pad=%dx%d s=%d)",

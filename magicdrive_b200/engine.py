@@ -622,19 +622,24 @@ class ControlNetEngine(_Net):
         return down, mid
 
 
-class VaeDecoderEngine:
-    """AutoencoderKL.decode for the 6 generated views (pipeline_bev_controlnet.py:100-112 -> autoencoder_kl.py:177-196 ->
-    vae.py:226-273): the step after the denoising path, built from the same operators (implicit-GEMM 3x3 convolutions,
-    single-kernel GroupNorm+SiLU, nearest x2).  The mid block's single-head attention is 512 wide — beyond the fused
+class _VaeEngine:
+    """The blocks the VAE's encoder and decoder share, on the same operators as the denoising path (implicit-GEMM 3x3
+    convolutions, single-kernel GroupNorm+SiLU).  The mid block's single-head attention is 512 wide — beyond the fused
     attention kernels' head dims — and runs as three tensor-core GEMMs per image around a row softmax:
     S = Q K^T (fp32, scaled), P = softmax(S) (bf16, key count padded to a K block), V^T = W_v X^T, O = P V + b_v."""
-
-    COUT_PAD = 8
 
     def __init__(self, cfg: arch.VaeConfig, sd, device):
         self.cfg, self.device = cfg, device
         self.W = _Weights(sd, device)
-        self.blocks = arch.vae_decoder_blocks(cfg)
+
+    def _conv(self, p):
+        """Conv2d `p` as a K64-packed bf16 matrix (the plain (tap, channel) layout when the input channels are a multiple
+        of 64, as in SD-1.5) and an fp32 bias."""
+        W = self.W
+        if p + ".w64" not in W.t:
+            W.t[p + ".w64"] = pack_conv_weight_k64(W.raw(p + ".weight").float())
+            W.t[p + ".b"] = _f32(W.raw(p + ".bias"))
+        return W.t[p + ".w64"], W.t[p + ".b"]
 
     def _resnet(self, p: str, x: FMap, cout: int) -> FMap:
         """ResnetBlock2D.forward with temb = None (resnet.py:590-640)."""
@@ -642,23 +647,22 @@ class VaeDecoderEngine:
         hw = x.h * x.w
         g1, b1 = W.norm(p + ".norm1")
         h = ops.groupnorm(x.data, x.c, x.c, x.n, hw, g1, b1, 1e-6, True, groups=g)
-        w1, c1 = W.conv(p + ".conv1")
+        w1, c1 = self._conv(p + ".conv1")
         h = ops.gemm_conv(h, w1, n_img=x.n, h_in=x.h, w_in=x.w, c0=x.c, lda0=x.c, n_out=cout, taps=3, pad=1, bias=c1)
         g2, b2 = W.norm(p + ".norm2")
         h = ops.groupnorm(h, cout, cout, x.n, hw, g2, b2, 1e-6, True, groups=g)
         res = x.data
         if x.c != cout:
-            ws, bs = W.conv(p + ".conv_shortcut")
+            ws, bs = self._conv(p + ".conv_shortcut")
             res = ops.gemm_conv(x.data, ws, n_img=x.n, h_in=x.h, w_in=x.w, c0=x.c, lda0=x.c, n_out=cout, bias=bs)
-        w2, c2 = W.conv(p + ".conv2")
+        w2, c2 = self._conv(p + ".conv2")
         out = ops.gemm_conv(h, w2, n_img=x.n, h_in=x.h, w_in=x.w, c0=cout, lda0=cout, n_out=cout, taps=3, pad=1, bias=c2,
                             residual=res, ldr=cout)
         return FMap(out, x.n, x.h, x.w, cout)
 
-    def _attention(self, x: FMap) -> FMap:
-        """Attention(heads=1, dim_head=C, GroupNorm, residual) of UNetMidBlock2D (unet_2d_blocks.py:433-446)."""
+    def _attention(self, a: str, x: FMap) -> FMap:
+        """Attention(heads=1, dim_head=C, GroupNorm, residual) `a` of UNetMidBlock2D (unet_2d_blocks.py:433-446)."""
         W, C, L = self.W, x.c, x.h * x.w
-        a = "decoder.mid_block.attentions.0"
         g, b = W.norm(a + ".group_norm")
         t = ops.groupnorm(x.data, C, C, x.n, L, g, b, 1e-6, False, groups=self.cfg.norm_num_groups)
         wq, bq = W.lin(a + ".to_q")
@@ -691,6 +695,17 @@ class VaeDecoderEngine:
         out = ops.linear(o, wo, bias=bo, residual=x.data)
         return FMap(out, x.n, x.h, x.w, C)
 
+
+class VaeDecoderEngine(_VaeEngine):
+    """AutoencoderKL.decode for the 6 generated views (pipeline_bev_controlnet.py:100-112 -> autoencoder_kl.py:177-196 ->
+    vae.py:226-273): the step after the denoising path, with nearest x2 upsampling between the up blocks."""
+
+    COUT_PAD = 8
+
+    def __init__(self, cfg: arch.VaeConfig, sd, device):
+        super().__init__(cfg, sd, device)
+        self.blocks = arch.vae_decoder_blocks(cfg)
+
     def decode(self, z_nhwc: torch.Tensor, n: int, h: int, w: int, scale: float = 1.0, to_unit_range: bool = False):
         """z_nhwc: fp32 [n*h*w, 4] latents (the denoiser's resident layout); `scale` multiplies them first
         (1 / scaling_factor).  Returns fp32 [n, 8h, 8w, 3] (with to_unit_range: image / 2 + 0.5 clamped to [0, 1])."""
@@ -706,14 +721,14 @@ class VaeDecoderEngine:
         x = ops.conv_direct(x, wd, bd, n=n, h=h, w=w, cin=lc, cout=c, k=3)
         x = FMap(x.reshape(n * h * w, c), n, h, w, c)
         x = self._resnet("decoder.mid_block.resnets.0", x, c)
-        x = self._attention(x)
+        x = self._attention("decoder.mid_block.attentions.0", x)
         x = self._resnet("decoder.mid_block.resnets.1", x, c)
         for _, resnets, up in self.blocks:
             for p, _, cout in resnets:
                 x = self._resnet(p, x, cout)
             if up:
                 u = ops.upsample_nearest(x.data, x.n, x.h, x.w, x.c, 2 * x.h, 2 * x.w)
-                wu, bu = W.conv(up)
+                wu, bu = self._conv(up)
                 out = ops.gemm_conv(u, wu, n_img=x.n, h_in=2 * x.h, w_in=2 * x.w, c0=x.c, lda0=x.c, n_out=x.c, taps=3, pad=1,
                                     bias=bu)
                 x = FMap(out, x.n, 2 * x.h, 2 * x.w, x.c)
@@ -730,6 +745,77 @@ class VaeDecoderEngine:
                             bias=bo, out_f32=True, out_scale=0.5 if to_unit_range else 1.0)
         img = img.reshape(x.n, x.h, x.w, self.COUT_PAD)[..., : cfg.out_channels]
         return img.clamp(0, 1) if to_unit_range else img
+
+
+class VaeEncoderEngine(_VaeEngine):
+    """AutoencoderKL.encode (autoencoder_kl.py:160-171 -> Encoder.forward, vae.py:108-149): camera images to the latent
+    moments, for given-view generation from real views (demo/run_cond_on_view.py:80-85).  mdb_fid_input turns the RGB
+    batch into conv_in's 8-channel bf16 operand (one partial K block per tap); each Downsample2D(padding=0), which pads
+    the bottom and right edge by one (resnet.py:199,213-217), is one stride-2 convolution with end padding 1; quant_conv
+    is folded into conv_out: W = Q W_out, b = Q b_out + b_q, composed in fp32 and rounded to bf16 once, so the moments
+    come out of one GEMM epilogue in fp32."""
+
+    def __init__(self, cfg: arch.VaeConfig, sd, device):
+        super().__init__(cfg, sd, device)
+        self.blocks = arch.vae_encoder_blocks(cfg)
+        self.moments = 2 * cfg.latent_channels
+        self.mpad = (self.moments + 7) // 8 * 8  # the kernel's N granularity
+
+    def _conv_in(self):
+        """conv_in with its RGB input channels zero-padded to the 8 that mdb_fid_input writes."""
+        W = self.W
+        if "encoder.conv_in.w8" not in W.t:
+            w = W.raw("encoder.conv_in.weight").float()
+            w = torch.cat([w, w.new_zeros((w.shape[0], 8 - w.shape[1], *w.shape[2:]))], 1)
+            W.t["encoder.conv_in.w8"] = pack_conv_weight_k64(w)
+            W.t["encoder.conv_in.b"] = _f32(W.raw("encoder.conv_in.bias"))
+        return W.t["encoder.conv_in.w8"], W.t["encoder.conv_in.b"]
+
+    def _conv_out(self, mean_scale: float):
+        """conv_out followed by the 1x1 quant_conv as one 3x3 filter; the mean rows also carry `mean_scale`."""
+        W, key = self.W, ("encoder.conv_out_q", float(mean_scale))
+        if key not in W.t:
+            w, b = W.raw("encoder.conv_out.weight").float(), W.raw("encoder.conv_out.bias").float()
+            q, bq = W.raw("quant_conv.weight").float()[:, :, 0, 0], W.raw("quant_conv.bias").float()
+            wf = torch.zeros((self.mpad, *w.shape[1:]), dtype=F32, device=w.device)
+            bf = torch.zeros((self.mpad,), dtype=F32, device=w.device)
+            wf[: self.moments] = torch.einsum("om,mchw->ochw", q, w)
+            bf[: self.moments] = q @ b + bq
+            lc = self.cfg.latent_channels
+            wf[:lc] *= mean_scale
+            bf[:lc] *= mean_scale
+            W.t[key] = (pack_conv_weight_k64(wf, dtype=W.fold_dtype), bf)
+        return W.t[key]
+
+    def encode(self, x: torch.Tensor, mean_scale: float = 1.0):
+        """x: (n, 3, H, W) fp32 or bf16 images in [-1, 1] on the device.  Returns (moments, h, w): fp32
+        [n*h*w, 2*latent_channels rounded up to 8] NHWC, mean channels first and multiplied by `mean_scale`, then logvar."""
+        cfg, W = self.cfg, self.W
+        n, cin, h, w = x.shape
+        if cin != 3:
+            raise ValueError(f"VaeEncoderEngine reads RGB images, got {cin} channels")
+        a = ops.fid_input(x, nhwc=False, quantize=False, normalize=False)  # bf16 [n*h*w, 8], channels 3..7 zero
+        wi, bi = self._conv_in()
+        c = cfg.block_out_channels[0]
+        x = FMap(ops.gemm_conv(a, wi, n_img=n, h_in=h, w_in=w, c0=8, lda0=8, n_out=c, taps=3, pad=1, bias=bi), n, h, w, c)
+        for _, resnets, down in self.blocks:
+            for p, _, cout in resnets:
+                x = self._resnet(p, x, cout)
+            if down:
+                wd, bd = self._conv(down)
+                ho, wo = (x.h - 2) // 2 + 1, (x.w - 2) // 2 + 1  # (h + 1 - 3) // 2 + 1 with the bottom / right pad
+                out = ops.gemm_conv(x.data, wd, n_img=x.n, h_in=x.h, w_in=x.w, c0=x.c, lda0=x.c, n_out=x.c, taps=3, stride=2,
+                                    pad=0, pad_h_end=1, pad_w_end=1, bias=bd)
+                x = FMap(out, x.n, ho, wo, x.c)
+        x = self._resnet("encoder.mid_block.resnets.0", x, x.c)
+        x = self._attention("encoder.mid_block.attentions.0", x)
+        x = self._resnet("encoder.mid_block.resnets.1", x, x.c)
+        g, b = W.norm("encoder.conv_norm_out")
+        hn = ops.groupnorm(x.data, x.c, x.c, x.n, x.h * x.w, g, b, 1e-6, True, groups=cfg.norm_num_groups)
+        wm, bm = self._conv_out(mean_scale)
+        m = ops.gemm_conv(hn, wm, n_img=x.n, h_in=x.h, w_in=x.w, c0=x.c, lda0=x.c, n_out=self.mpad, taps=3, pad=1, bias=bm,
+                          out_f32=True)
+        return m, x.h, x.w
 
 
 class TextEncoderEngine:

@@ -8,6 +8,7 @@ magicdrive/networks/unet_addon_rawbox.py:707-724,921-932), plus the helper metho
 kernels; inputs must be CUDA tensors — there is no CPU path (ops raise).
 """
 import json
+import math
 import logging
 import os
 from collections import OrderedDict
@@ -18,7 +19,7 @@ import torch
 import torch.nn as nn
 
 from . import arch, ops
-from .engine import ControlNetEngine, InceptionEngine, TextEncoderEngine, UNetEngine, VaeDecoderEngine
+from .engine import ControlNetEngine, InceptionEngine, TextEncoderEngine, UNetEngine, VaeDecoderEngine, VaeEncoderEngine
 
 BF16, F32 = torch.bfloat16, torch.float32
 
@@ -43,7 +44,7 @@ class _Config(dict):
     __getattr__ = dict.__getitem__
 
 
-def _register_tree(root: nn.Module, shapes: "OrderedDict[str, tuple]", dtype=F32):
+def _register_tree(root: nn.Module, shapes: "OrderedDict[str, tuple]", dtype=F32, device=None):
     """Create nested nn.Modules so that parameter names equal the reference checkpoint keys."""
     for key, shape in shapes.items():
         parts = key.split(".")
@@ -52,7 +53,7 @@ def _register_tree(root: nn.Module, shapes: "OrderedDict[str, tuple]", dtype=F32
             if name not in mod._modules:
                 mod.add_module(name, nn.Module())
             mod = mod._modules[name]
-        t = torch.empty(shape, dtype=dtype)
+        t = torch.empty(shape, dtype=dtype, device=device)
         if key in arch.BUFFER_KEYS:
             mod.register_buffer(parts[-1], t)
         else:
@@ -428,12 +429,67 @@ class DecoderOutput:  # diffusers/models/vae.py:27-36
         return (self.sample,)[i]
 
 
+class DiagonalGaussianDistribution:
+    """diffusers' posterior of AutoencoderKL.encode (vae.py:397-441) over moments (n, 2 * latent_channels, h, w): mean and
+    logvar halves, logvar clamped to [-30, 20], std, var; `sample(generator)` draws its noise as randn_tensor does
+    (utils/torch_utils.py:36-77): a CPU generator draws on the CPU, then the noise moves to the moments' device."""
+
+    def __init__(self, parameters: torch.Tensor, deterministic: bool = False):
+        self.parameters = parameters
+        self.mean, self.logvar = torch.chunk(parameters, 2, dim=1)
+        self.logvar = torch.clamp(self.logvar, -30.0, 20.0)
+        self.deterministic = deterministic
+        self.std = torch.exp(0.5 * self.logvar)
+        self.var = torch.exp(self.logvar)
+        if deterministic:
+            self.var = self.std = torch.zeros_like(self.mean)
+
+    def sample(self, generator=None) -> torch.Tensor:
+        shape, dev, dt = self.mean.shape, self.parameters.device, self.parameters.dtype
+        if isinstance(generator, list):
+            noise = torch.cat([torch.randn((1, *shape[1:]), generator=g, device=g.device, dtype=dt) for g in generator])
+        elif generator is not None:
+            if generator.device.type != dev.type and generator.device.type != "cpu":
+                raise ValueError(f"Cannot generate a {dev} tensor from a generator of type {generator.device.type}.")
+            noise = torch.randn(shape, generator=generator, device=generator.device, dtype=dt)
+        else:
+            noise = torch.randn(shape, device=dev, dtype=dt)
+        return self.mean + self.std * noise.to(dev)
+
+    def mode(self) -> torch.Tensor:
+        return self.mean
+
+    def kl(self, other=None):
+        if self.deterministic:
+            return torch.Tensor([0.0])
+        if other is None:
+            return 0.5 * torch.sum(self.mean ** 2 + self.var - 1.0 - self.logvar, dim=[1, 2, 3])
+        return 0.5 * torch.sum((self.mean - other.mean) ** 2 / other.var + self.var / other.var - 1.0 - self.logvar
+                               + other.logvar, dim=[1, 2, 3])
+
+    def nll(self, sample, dims=(1, 2, 3)):
+        if self.deterministic:
+            return torch.Tensor([0.0])
+        return 0.5 * torch.sum(math.log(2.0 * math.pi) + self.logvar + (sample - self.mean) ** 2 / self.var, dim=list(dims))
+
+
+class AutoencoderKLOutput:  # diffusers/models/autoencoder_kl.py:27-37
+    def __init__(self, latent_dist):
+        self.latent_dist = latent_dist
+
+    def __getitem__(self, i):
+        return (self.latent_dist,)[i]
+
+
 class AutoencoderKL(_B200Module):
-    """Decoder half of diffusers' AutoencoderKL (models/autoencoder_kl.py) for the pipeline's `decode_latents`
-    (pipeline_bev_controlnet.py:100-112): same constructor kwargs and checkpoint key names (`decoder.*`,
-    `post_quant_conv.*`; `encoder.*` / `quant_conv.*` of a full checkpoint are accepted and ignored), `.config.scaling_factor`
-    and `.config.block_out_channels` as the pipeline reads them (pipeline_controlnet.py:130-179), `decode(z).sample`.
-    Encoding is not on the path and raises."""
+    """diffusers' AutoencoderKL (models/autoencoder_kl.py) for the pipeline's `decode_latents` (pipeline_bev_controlnet.py:
+    100-112) and the given-view demo's `vae.encode(...)` (demo/run_cond_on_view.py:80-85): same constructor kwargs and
+    checkpoint key names, `.config.scaling_factor` and `.config.block_out_channels` as the pipeline reads them
+    (pipeline_controlnet.py:130-179), `decode(z).sample` and `encode(x).latent_dist`.
+    The decoder (`decoder.*`, `post_quant_conv.*`) is always present.  The encoder (`encoder.*`, `quant_conv.*`) is kept
+    when a state dict holds its complete set for this config; a decoder-only state dict, or one with only part of the
+    encoder, loads the decoder alone (the encoder keys are ignored) and `encode` raises NotImplementedError naming what is
+    missing."""
 
     def __init__(self, **kwargs):
         super().__init__()
@@ -442,23 +498,41 @@ class AutoencoderKL(_B200Module):
         if cfg.act_fn != "silu" or any(t != "UpDecoderBlock2D" for t in cfg.up_block_types):
             raise ValueError("only the SD-1.5 AutoencoderKL layout (UpDecoderBlock2D, silu) is implemented")
         self._init_common(cfg, arch.vae_decoder_param_shapes(cfg), extra)
+        self._encoder_missing = sorted(arch.vae_encoder_param_shapes(cfg))  # keys encode() still needs
+        self._enc_engine = None
         self.training = False
 
     _OLD_ATTN = {"query": "to_q", "key": "to_k", "value": "to_v", "proj_attn": "to_out.0"}  # pre-0.17 checkpoint names
+    _ENCODER_PREFIXES = ("encoder.", "quant_conv.")
 
     def load_state_dict(self, state_dict, strict=True, **kw):
         sd = {}
         for k, v in state_dict.items():
-            if k.startswith(("encoder.", "quant_conv.")):
-                continue
             parts = k.split(".")
             if "attentions" in parts and parts[-2] in self._OLD_ATTN:  # attention_processor.py:_from_deprecated_attn_block
                 k = ".".join(parts[:-2] + [self._OLD_ATTN[parts[-2]], parts[-1]])
             sd[k] = v
+        enc_shapes = arch.vae_encoder_param_shapes(self.arch_cfg)
+        missing = sorted(k for k in enc_shapes if k not in sd)
+        for name in ("encoder", "quant_conv"):  # the encoder is re-registered below only if this state dict completes it
+            self._modules.pop(name, None)
+        if missing:
+            sd = {k: v for k, v in sd.items() if not k.startswith(self._ENCODER_PREFIXES)}
+        else:
+            p = next(self.parameters())
+            _register_tree(self, enc_shapes, dtype=p.dtype, device=p.device)
+        self._encoder_missing = missing
+        self._enc_engine = None
         return super().load_state_dict(sd, strict=strict, **kw)
 
-    use_cuda_graph = True  # decode_latents replays one captured graph per shape
+    def _apply(self, fn, *a, **k):
+        r = super()._apply(fn, *a, **k)
+        self._enc_engine = None
+        return r
+
+    use_cuda_graph = True  # decode_latents / encode_latents replay one captured graph per shape
     _decode_graphs: dict = {}
+    _encode_graphs: dict = {}
 
     def engine(self) -> VaeDecoderEngine:
         eng = self._get_engine(VaeDecoderEngine)
@@ -466,8 +540,66 @@ class AutoencoderKL(_B200Module):
             self._decode_graphs, self._graphs_for = {}, eng
         return eng
 
-    def encode(self, *a, **k):
-        raise NotImplementedError("AutoencoderKL.encode is not on the generation path (SURVEY.md §2.1); only decode is built")
+    def encoder_engine(self) -> VaeEncoderEngine:
+        if self._encoder_missing:
+            shown = ", ".join(self._encoder_missing[:4]) + (", ..." if len(self._encoder_missing) > 4 else "")
+            raise NotImplementedError(
+                f"AutoencoderKL.encode needs the encoder.* and quant_conv.* weights of this config; the loaded state dict "
+                f"lacks {len(self._encoder_missing)} of them ({shown})")
+        if any(t != "DownEncoderBlock2D" for t in self.arch_cfg.down_block_types) or self.arch_cfg.in_channels != 3:
+            raise NotImplementedError("AutoencoderKL.encode implements the SD-1.5 encoder layout (RGB in, DownEncoderBlock2D)")
+        if self._enc_engine is None:
+            dev = self.device
+            if dev.type != "cuda":
+                raise ops._lib.MdbError(f"AutoencoderKL.encode runs only on a CUDA (sm_90a) device; parameters are on {dev}")
+            self._enc_engine = VaeEncoderEngine(self.arch_cfg, dict(self.state_dict()), dev)
+            self._encode_graphs = {}
+        return self._enc_engine
+
+    @torch.no_grad()
+    def encode(self, x: torch.Tensor, return_dict: bool = True):
+        """x: (n, 3, H, W) images in [-1, 1] on the device, any float dtype (fp32 and bf16 are read directly) ->
+        AutoencoderKLOutput(latent_dist=DiagonalGaussianDistribution) over (n, 2 * latent_channels, h, w) moments in x's
+        dtype, h = H / 8 for the SD-1.5 layout (autoencoder_kl.py:160-171)."""
+        eng = self.encoder_engine()
+        xin = x if x.dtype in (F32, BF16) else x.float()
+        m, h, w = eng.encode(xin.to(self.device).contiguous())
+        moments = m.view(x.shape[0], h, w, -1)[..., : eng.moments].permute(0, 3, 1, 2).to(x.dtype)
+        dist = DiagonalGaussianDistribution(moments)
+        return AutoencoderKLOutput(dist) if return_dict else (dist,)
+
+    @torch.no_grad()
+    def encode_latents(self, pixel_values: torch.Tensor) -> torch.Tensor:
+        """The given-view demo's `vae.encode(rearrange(pixel_values, "b n c h w -> (b n) c h w")).latent_dist.mean *
+        scaling_factor` (run_cond_on_view.py:80-85): (b, n_cam, 3, H, W) images in [-1, 1] -> (b, n_cam, latent_channels,
+        H/8, W/8) fp32 latents, ready for the denoiser's `conditional_latents`.  scaling_factor is folded into conv_out."""
+        b, n_cam = pixel_values.shape[:2]
+        eng = self.encoder_engine()
+        x = pixel_values.to(self.device).reshape(b * n_cam, *pixel_values.shape[2:])
+        x = (x if x.dtype in (F32, BF16) else x.float()).contiguous()
+        lc, sf = self.arch_cfg.latent_channels, float(self.config["scaling_factor"])
+        run = lambda xx: eng.encode(xx, mean_scale=sf)
+        if not (self.use_cuda_graph and x.is_cuda):
+            m, h, w = run(x)
+        else:
+            # the encode of a given shape and dtype is one CUDA graph on resident input / output buffers (eager once to size
+            # scratch)
+            key = (id(eng), tuple(x.shape), x.dtype)
+            g = self._encode_graphs.get(key)
+            if g is None:
+                xin = x.clone()
+                run(xin)
+                torch.cuda.synchronize()
+                graph = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(graph):
+                    out = run(xin)
+                g = self._encode_graphs[key] = (graph, xin, out)
+            graph, xin, (out, h, w) = g
+            xin.copy_(x)
+            graph.replay()
+            m = out.clone()
+        lat = m.view(b, n_cam, h, w, -1)[..., :lc]
+        return lat.permute(0, 1, 4, 2, 3).contiguous()
 
     @torch.no_grad()
     def decode(self, z: torch.Tensor, return_dict: bool = True):

@@ -127,11 +127,14 @@ def gemm_conv(a0: torch.Tensor, w: torch.Tensor, *, n_img: int, h_in: int, w_in:
               force_block_n: int = 0, force_splits: int = 0, allow_split_k: bool = True, kernel_variant: int = 0,
               ln: Optional["RowStats"] = None, ln_colsum: Optional[torch.Tensor] = None, ln_eps: float = 1e-5,
               emit_stats: bool = False, quick_gelu: bool = False, relu: bool = False, taps_h: Optional[int] = None,
-              taps_w: Optional[int] = None, pad_h: Optional[int] = None, pad_w: Optional[int] = None):
+              taps_w: Optional[int] = None, pad_h: Optional[int] = None, pad_w: Optional[int] = None,
+              pad_h_end: int = 0, pad_w_end: int = 0):
     """wgmma GEMM / implicit-GEMM conv (mdb_gemm_conv).  `a0` (and `a1`) are NHWC bf16 buffers whose pixel
     stride is lda* elements; `w` is bf16 [n_out, taps_h*taps_w*K64] with K64 = c0+c1, each rounded up to 64
     (params.pack_conv_weight_k64; the plain (tap, channel) layout when c0 and c1 are multiples of 64).
     `taps` / `pad` give a square filter; taps_h, taps_w, pad_h, pad_w override them per dimension (1x7, 7x1, ...).
+    pad_h_end / pad_w_end: extra zero rows below / columns right of the image (F.pad(x, (0, pad_w_end, 0, pad_h_end))
+    before the convolution, as the VAE encoder's Downsample2D does).
     relu: out = max(0, linear epilogue value) (a BatchNorm folded into w / bias, then ReLU).
     ln / ln_colsum: fold a LayerNorm of the rows of `a0` into this GEMM (`ln` = the RowStats the producer of `a0`
     emitted, `w` pre-multiplied by gamma, `bias` = beta-term + bias).  emit_stats: also return the RowStats of the
@@ -143,9 +146,9 @@ def gemm_conv(a0: torch.Tensor, w: torch.Tensor, *, n_img: int, h_in: int, w_in:
     ph = pad if pad_h is None else pad_h
     pw = pad if pad_w is None else pad_w
     if h_out is None:
-        h_out = (h_in + 2 * ph - th) // stride + 1
+        h_out = (h_in + 2 * ph + pad_h_end - th) // stride + 1
     if w_out is None:
-        w_out = (w_in + 2 * pw - tw) // stride + 1
+        w_out = (w_in + 2 * pw + pad_w_end - tw) // stride + 1
     pixels = n_img * h_out * w_out
     width = n_out // 2 if geglu else n_out
     if out is None:
@@ -160,6 +163,7 @@ def gemm_conv(a0: torch.Tensor, w: torch.Tensor, *, n_img: int, h_in: int, w_in:
     d.w, d.n_out = _ptr(w), n_out
     d.taps_h, d.taps_w = th, tw
     d.stride, d.pad_h, d.pad_w = stride, ph, pw
+    d.pad_h_end, d.pad_w_end = pad_h_end, pad_w_end
     d.h_out, d.w_out = h_out, w_out
     d.bias = _ptr(bias)
     d.rowbias = _ptr(rowbias)
