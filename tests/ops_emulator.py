@@ -146,11 +146,16 @@ def add(a, b):
     return _act(a.float() + b.float())
 
 
+def nearest_index(n_in, n_out):
+    """ATen's nearest source index: min(floor(dst * scale), n_in - 1) with scale = n_in / n_out and the product in float32.
+    Not the exact floor(dst * n_in / n_out): at 26 -> 44, output row 22 reads row 12, not 13."""
+    scale = torch.tensor(n_in, dtype=torch.float32) / torch.tensor(n_out, dtype=torch.float32)
+    return (torch.arange(n_out, dtype=torch.float32) * scale).floor().long().clamp_max(n_in - 1)
+
+
 def upsample_nearest(x, n, h, w, c, ho, wo):
     xi = x.float().reshape(n, h, w, c)
-    iy = torch.div(torch.arange(ho) * h, ho, rounding_mode="floor")
-    ix = torch.div(torch.arange(wo) * w, wo, rounding_mode="floor")
-    return xi[:, iy][:, :, ix].reshape(n * ho * wo, c).contiguous()
+    return xi[:, nearest_index(h, ho)][:, :, nearest_index(w, wo)].reshape(n * ho * wo, c).contiguous()
 
 
 def adaptive_avgpool(x, n, h, w, c, ho, wo, silu=False):
