@@ -1,6 +1,6 @@
 """CLIP text encoder without a GPU: the fp32 oracle against the transformers fixtures, and the real host code (weight
-packing, layer sequencing, pooling, CLIPTextModel, the denoiser's `prompt=`) run through torch restatements of the
-operators (tests/ops_emulator.py plus, registered here, the three operators the text encoder adds)."""
+packing, layer sequencing, pooling, CLIPTextModel, the denoiser's `prompt=`) run through the torch restatements of the
+operators in tests/ops_emulator.py."""
 import json
 from dataclasses import asdict
 from types import SimpleNamespace
@@ -8,7 +8,7 @@ from types import SimpleNamespace
 import pytest
 import torch
 
-from magicdrive_b200 import arch, engine, models, ops
+from magicdrive_b200 import arch, engine, models
 from oracle.clip_text import TINY, clip_text_forward, draw_weights
 from tests import ops_emulator
 from tests.common import golden, tiny_configs, tiny_state_dicts
@@ -22,52 +22,10 @@ def _rel(a, b):
     return ((a.float() - b.float()).abs().max() / b.float().abs().max()).item()
 
 
-# ------------------------------------------------------------------------------------------- the three new operators
-def _attention_causal(q, k, v, *, b, heads, l, d, ldq, ldk, ldv, scale, out=None):
-    c = heads * d
-    assert q.stride(0) == ldq and k.stride(0) == ldk and v.stride(0) == ldv
-    qh, kh, vh = (t[:, :c].float().reshape(b, l, heads, d).transpose(1, 2) for t in (q, k, v))
-    mask = torch.full((l, l), float("-inf")).triu(1)
-    o = torch.softmax(qh @ kh.transpose(-1, -2) * scale + mask, -1) @ vh
-    res = ops_emulator._act(o.transpose(1, 2).reshape(b * l, c))
-    if out is not None:
-        out[:, :c] = res
-        return out
-    return res
-
-
-def _clip_embed(ids, tok, pos, out=None):
-    n, ln = ids.shape
-    bad = (ids < 0) | (ids >= tok.shape[0])
-    x = tok.float()[ids.clamp(0, tok.shape[0] - 1).long()] + pos.float()[:ln][None]
-    x = torch.where(bad[..., None], torch.full_like(x, float("nan")), x)
-    x = ops_emulator._act(x.reshape(n * ln, -1))
-    stats = torch.stack([x.sum(1), (x * x).sum(1)], -1)[:, None]
-    return x, ops.RowStats(stats.contiguous(), 1)
-
-
-def _gemm_conv(*a, quick_gelu=False, **k):
-    emit = k.get("emit_stats", False)
-    assert not (quick_gelu and (emit or k.get("residual") is not None))
-    r = ops_emulator.gemm_conv(*a, **k)
-    return r * torch.sigmoid(1.702 * r) if quick_gelu else r
-
-
-def _linear(x, w, bias=None, residual=None, out=None, ldo=None, geglu=False, out_f32=False, out_scale=1.0, **kw):
-    m, k = x.shape
-    return _gemm_conv(x, w, n_img=1, h_in=1, w_in=m, c0=k, lda0=x.stride(0), n_out=w.shape[0], bias=bias,
-                      residual=residual, ldr=(residual.stride(0) if residual is not None else 0), out=out, ldo=ldo,
-                      geglu=geglu, out_f32=out_f32, out_scale=out_scale, **kw)
-
-
 @pytest.fixture
 def emulated(monkeypatch):
     ops_emulator.install(monkeypatch)
     monkeypatch.setattr(engine._Weights, "fold_dtype", torch.float32)
-    for name, fn in (("attention_causal", _attention_causal), ("clip_embed", _clip_embed), ("gemm_conv", _gemm_conv),
-                     ("linear", _linear)):
-        assert hasattr(ops, name), name
-        monkeypatch.setattr(ops, name, fn)
 
 
 def _model(cfg_kwargs, sd):

@@ -1,18 +1,18 @@
 """Host logic of pipeline.BEVControlNetDenoiser on CPU: scheduler tables (DDIM / UniPC), multistep history handling, the two
 given-view modes, call ordering -- checked against fixtures produced by the REFERENCE pipelines themselves.
 
-There is no GPU in the build container and the product has no CPU path, so for THIS test only the CUDA engines and the
-elementwise operators the denoiser launches are replaced by stand-ins that restate each operator's documented semantics
-(include/magicdrive_b200.h) in torch; the engines' arithmetic is the oracle's (same stand-ins as
-tests/test_dropin_reference_pipeline_cpu.py).  The real kernels are compared with the same fixtures in
+There is no GPU in the build container and the product has no CPU path, so the operators the denoiser launches run on
+their torch restatements (tests/ops_emulator.py) and the CUDA engines are replaced by stand-ins whose arithmetic is the
+oracle's (the same stand-ins as tests/test_dropin_reference_pipeline_cpu.py).  The real kernels are compared with the same fixtures in
 tests/test_model_gpu.py and tests/test_zz_sampling_gpu.py."""
 from dataclasses import asdict
 
 import pytest
 import torch
 
-from magicdrive_b200 import models, ops
+from magicdrive_b200 import models
 from magicdrive_b200.pipeline import BEVControlNetDenoiser
+from tests import ops_emulator
 from tests.common import golden, tiny_configs, tiny_state_dicts
 from tests.test_dropin_reference_pipeline_cpu import _FakeControlNetEngine, _FakeUNetEngine
 
@@ -30,44 +30,11 @@ class _ControlNetEngine(_FakeControlNetEngine):
         return torch.zeros(len(tt), 8)
 
 
-def _cfg_combine(eps, cfg, guidance, c, npix):
-    e = eps[:, :c].float()
-    return e[:npix] + guidance * (e[npix:] - e[:npix]) if cfg else e
-
-
-def _cfg_ddim_step(eps, latents, coef, cfg, guidance, c=4):
-    latents.copy_(coef[0] * latents + coef[1] * _cfg_combine(eps, cfg, guidance, c, latents.shape[0]))
-    return latents
-
-
-def _cfg_unipc_step(eps, latents, last, m0, m1, coef, cfg, guidance, c=4):
-    e, x = _cfg_combine(eps, cfg, guidance, c, latents.shape[0]), latents.clone()
-    x0 = coef[0] * x + coef[1] * e
-    xc = coef[2] * last + coef[3] * m0 + coef[4] * m1 + coef[5] * x0 if coef[9] != 0 else x
-    latents.copy_(coef[6] * xc + coef[7] * x0 + coef[8] * m0)
-    last.copy_(xc)
-    m1.copy_(m0)
-    m0.copy_(x0)
-    return latents
-
-
-def _pin_views(dst, a, b, coef, view_mask, rows_per_view, c=4):
-    sel = view_mask.bool().repeat_interleave(rows_per_view)
-    dst[sel, :c] = (coef[0] * a[sel] if a is not None else 0) + coef[1] * b[sel]
-    return dst
-
-
 @pytest.fixture
 def cpu_standins(monkeypatch):
+    ops_emulator.install(monkeypatch)
     monkeypatch.setattr(models, "UNetEngine", _UNetEngine)
     monkeypatch.setattr(models, "ControlNetEngine", _ControlNetEngine)
-    monkeypatch.setattr(models._B200Module, "_get_engine",
-                        lambda self, cls_: self.__dict__.setdefault("_eng", cls_(self.arch_cfg, dict(self.state_dict()), "cpu")))
-    monkeypatch.setattr(ops, "pack_latents", lambda x, cpad=64, repeat=1: torch.nn.functional.pad(x.float(), (0, cpad - x.shape[1])).repeat(repeat, 1))
-    monkeypatch.setattr(ops, "f32_to_bf16", lambda x: x)
-    monkeypatch.setattr(ops, "cfg_ddim_step", _cfg_ddim_step)
-    monkeypatch.setattr(ops, "cfg_unipc_step", _cfg_unipc_step)
-    monkeypatch.setattr(ops, "pin_views", _pin_views)
 
 
 def _denoiser(seed, scheduler):

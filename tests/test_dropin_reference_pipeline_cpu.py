@@ -2,18 +2,19 @@
 (imported through oracle/ref_shim.py) and its unmodified `__call__` drives them: CFG batching, add_uncond_to_kwargs,
 uncond_cam_param, the 5-D / 4-D reshapes, `.sample`, `return_dict=False` tuples, `.config.in_channels`, `.dtype`.
 
-There is no GPU in the build container and the product has no CPU path, so for THIS test only the CUDA engine and the
-five layout/dtype ops the module wrappers call are replaced by oracle-backed stand-ins (NHWC in / NHWC out, like the
-real engines).  What is exercised is the host logic of magicdrive_b200.models against the reference pipeline; the
+There is no GPU in the build container and the product has no CPU path, so for THIS test the CUDA engines are replaced by
+oracle-backed stand-ins (NHWC in / NHWC out, like the real engines) and the layout / dtype operators the module wrappers
+call run on their torch restatements (tests/ops_emulator.py).  What is exercised is the host logic of magicdrive_b200.models against the reference pipeline; the
 arithmetic of the real engines is covered by tests/test_model_gpu.py.  Skipped when /root/reference is absent."""
 from dataclasses import asdict
 
 import pytest
 import torch
 
-from magicdrive_b200 import models, ops
+from magicdrive_b200 import models
 from oracle import ref_shim
 from oracle import torch_oracle as O
+from tests import ops_emulator
 from tests.common import golden, tiny_configs, tiny_state_dicts
 
 pytestmark = pytest.mark.skipif(not ref_shim.available(), reason="reference tree not mounted")
@@ -85,14 +86,9 @@ class _FakeControlNetEngine:
 
 @pytest.fixture
 def cpu_standins(monkeypatch):
+    ops_emulator.install(monkeypatch)
     monkeypatch.setattr(models, "UNetEngine", _FakeUNetEngine)
     monkeypatch.setattr(models, "ControlNetEngine", _FakeControlNetEngine)
-    monkeypatch.setattr(models._B200Module, "_get_engine",
-                        lambda self, cls_: self.__dict__.setdefault("_eng", cls_(self.arch_cfg, dict(self.state_dict()), "cpu")))
-    monkeypatch.setattr(ops, "nchw_to_nhwc", lambda x: x.permute(0, 2, 3, 1).reshape(-1, x.shape[1]).contiguous())
-    monkeypatch.setattr(ops, "pack_latents", lambda x, cpad=64, repeat=1: torch.nn.functional.pad(x.float(), (0, cpad - x.shape[1])).repeat(repeat, 1))
-    monkeypatch.setattr(ops, "nhwc_to_nchw", lambda x, n, c, h, w, dtype=torch.float32: x.reshape(n, h, w, c).permute(0, 3, 1, 2).to(dtype))
-    monkeypatch.setattr(ops, "f32_to_bf16", lambda x: x)
 
 
 @torch.no_grad()

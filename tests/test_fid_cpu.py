@@ -1,6 +1,6 @@
 """FID host side without a GPU: the Fréchet distance and statistics, the InceptionV3 wrapper's names, loading and
 rejections, and the real InceptionEngine host code (BatchNorm folding, K64 packing, column-slice wiring) through
-tests/fid_emulator.py against the fp32 oracle (oracle/fid_inception.py)."""
+tests/ops_emulator.py against the fp32 oracle (oracle/fid_inception.py)."""
 import numpy as np
 import pytest
 import torch
@@ -10,7 +10,7 @@ from magicdrive_b200 import arch, engine, fid
 from magicdrive_b200.engine import InceptionEngine
 from magicdrive_b200.models import InceptionV3
 from oracle import fid_inception as fid_oracle
-from tests import fid_emulator
+from tests import ops_emulator
 
 
 def _direct_fid(mu1, s1, mu2, s2):
@@ -126,7 +126,7 @@ def test_constructor_rejections():
 
 @pytest.mark.parametrize("size,resize", [((299, 299), True), ((97, 131), True), ((150, 171), False)])
 def test_engine_host_logic_through_emulated_ops(monkeypatch, size, resize):
-    fid_emulator.install(monkeypatch)
+    ops_emulator.install(monkeypatch)
     monkeypatch.setattr(engine._Weights, "fold_dtype", torch.float32)  # the fold's algebra to fp32, apart from bf16 storage
     sd = arch.inception_synthetic_state_dict(3, seed=2)
     eng = InceptionEngine(sd, torch.device("cpu"))

@@ -1,8 +1,39 @@
-"""tests/ops_emulator.py against torch where its restatement has a rule of its own to get right (CPU)."""
+"""tests/ops_emulator.py on the CPU: it restates exactly the operators of ops.py that launch a kernel, with their signatures,
+and against torch where its restatement has a rule of its own to get right."""
+import inspect
+
+import pytest
 import torch
 import torch.nn.functional as F
 
+from magicdrive_b200 import ops
 from tests import ops_emulator as E
+
+
+def _launching_operators():
+    """The functions of ops.py that call into the library, apart from the peer barrier and the launch-mode switch."""
+    fns = {n for n, f in inspect.getmembers(ops, inspect.isfunction)
+           if f.__module__ == ops.__name__ and "_lib.lib()" in inspect.getsource(f)}
+    return fns - {"peer_barrier", "pdl_region"}
+
+
+def _params(fn):
+    return [(p.name, p.kind, p.default) for p in inspect.signature(fn).parameters.values()]
+
+
+def test_emulated_names_are_the_launching_operators():
+    assert set(E.EMULATED) == _launching_operators() and len(E.EMULATED) == len(set(E.EMULATED))
+
+
+@pytest.mark.parametrize("name", E.EMULATED)
+def test_emulated_signature_equals_ops(name):
+    assert _params(getattr(E, name)) == _params(getattr(ops, name))
+
+
+def test_unknown_keyword_raises_type_error():
+    for name in E.EMULATED:
+        with pytest.raises(TypeError, match="unexpected keyword argument 'not_an_argument'"):
+            getattr(E, name)(not_an_argument=1)
 
 
 def _exact_floor_differs(n_in, n_out):

@@ -1,6 +1,6 @@
 """Camera rigs other than nuScenes' six-camera ring (neighboring_view_pair of any size, any neighbour count per view) on CPU:
 the oracle against the reference's own outputs (tests/golden/tiny_rigs.pt, oracle/make_golden_rigs.py), the engine's host
-side through tests/rigs_emulator.py against the oracle, and the constructor / view-sharding validation."""
+side through tests/ops_emulator.py against the oracle, and the constructor / view-sharding validation."""
 from dataclasses import asdict, replace
 
 import pytest
@@ -9,7 +9,7 @@ import torch
 from magicdrive_b200 import arch, models
 from magicdrive_b200.dist import ShardPlan
 from oracle import torch_oracle as O
-from tests import rigs_emulator
+from tests import ops_emulator
 from tests.common import golden, rel_l2, tiny_configs
 
 RIGS = ["chain5_add", "ring5_concat", "ring8_3_add", "six_empty_add"]
@@ -22,7 +22,7 @@ def _bf16_exact(sd):
 
 @pytest.fixture
 def emulated(monkeypatch):
-    rigs_emulator.install(monkeypatch)
+    ops_emulator.install(monkeypatch)
     from magicdrive_b200 import engine
     monkeypatch.setattr(engine._Weights, "fold_dtype", torch.float32)
 

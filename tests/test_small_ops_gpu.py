@@ -39,6 +39,7 @@ from oracle import input_prep as OP  # noqa: E402  (checker only)
 from tests.common import record  # noqa: E402
 from tests.test_kernel_edges_gpu import _FILL, BF16, F32, F64, G, _bf, _gen  # noqa: E402
 from tests.test_kernel_edges_gpu import Guarded as _Guarded  # noqa: E402
+from tests.test_kernel_edges_gpu import _attn_close, _close, _close_f32  # noqa: E402
 
 I32, I64, U8 = torch.int32, torch.int64, torch.uint8
 INVALID, UNSUPPORTED = -1, -3
@@ -737,14 +738,16 @@ def test_pdl_decoder_pipeline_bitwise(cuda_lib, monkeypatch):
 # ------------------------------------------------------------------------------------------------------ emulator vs kernels
 def test_ops_emulator_agrees_with_the_kernels(cuda_lib, monkeypatch):
     """tests/ops_emulator.py (the CPU restatement the host tests run on) against the kernels, with its bf16 rounding of
-    activations on, for every operator of this file it restates: bitwise where the kernel is exact, else within the
-    operator's bound above."""
+    activations on, for every operator of this file it restates and one case per semantic of the GEMM, attention and FID /
+    text-encoder operators: bitwise where the kernel is exact, else within the operator's bound above, one bf16 rounding
+    step for the GEMM (test_kernel_edges_gpu._close) and xformers' bf16 tolerance for attention."""
     from tests import ops_emulator as E
     monkeypatch.setattr(E, "ROUND_ACTIVATIONS", True)
     g = _gen(15)
     cpu = lambda t: None if t is None else t.cpu()  # noqa: E731
     assert {"add", "upsample_nearest", "nchw_to_nhwc", "nhwc_to_nchw", "f32_to_bf16", "pack_latents", "cfg_ddim_step",
-            "cfg_unipc_step", "pin_views", "timestep_embedding", "fourier_embed", "linear_small"} <= set(E.EMULATED)
+            "cfg_unipc_step", "pin_views", "timestep_embedding", "fourier_embed", "linear_small", "gemm_conv", "attention",
+            "attention_multi", "attention_causal", "pool2d", "fid_input", "clip_embed"} <= set(E.EMULATED)
 
     def same(dev, emu, what):
         _same(dev.cpu().to(emu.dtype).reshape(emu.shape), emu, f"emulator {what}")
@@ -810,3 +813,84 @@ def test_ops_emulator_agrees_with_the_kernels(cuda_lib, monkeypatch):
     _, bound = _linear_small_ref(h, wl, bl, True, True)
     _within("emulator linear_small", E.linear_small(cpu(h), cpu(wl), cpu(bl), True, True),
             ops.linear_small(h, wl, bl, True, True).cpu().to(F64), bound.cpu(), "linear_small")
+
+    # gemm_conv: two sources with K tails (80 + 40 channels), a 1x7 filter and ReLU into a column slice; end padding
+    from magicdrive_b200.params import pack_conv_weight_k64
+    x0, x1 = _bf(torch.randn(2 * 9 * 11, 88, device="cuda", generator=g)), _bf(torch.randn(2 * 9 * 11, 40, device="cuda", generator=g))
+    wk = pack_conv_weight_k64(torch.randn(64, 120, 1, 7, device="cuda", generator=g) / math.sqrt(840), [80, 40])
+    bk = torch.randn(64, device="cuda", generator=g)
+    conv = dict(n_img=2, h_in=9, w_in=11, c0=80, lda0=88, c1=40, lda1=40, n_out=64, taps_h=1, taps_w=7, pad_h=0, pad_w=3,
+                relu=True)
+    dev = ops.gemm_conv(x0, wk, a1=x1, bias=bk, out=torch.zeros(198, 80, dtype=BF16, device="cuda")[:, 8:72], ldo=80, **conv)
+    emu = E.gemm_conv(cpu(x0), cpu(wk), a1=cpu(x1), bias=cpu(bk), out=torch.zeros(198, 80)[:, 8:72], ldo=80, **conv)
+    _close(dev, emu.cuda(), "emulator gemm_conv 1x7 two sources relu")
+    xe = _bf(torch.randn(2 * 13 * 17, 64, device="cuda", generator=g))
+    we = pack_conv_weight_k64(torch.randn(96, 64, 3, 3, device="cuda", generator=g) / 24)
+    conv = dict(n_img=2, h_in=13, w_in=17, c0=64, lda0=64, n_out=96, taps=3, stride=2, pad=0, pad_h_end=1, pad_w_end=1)
+    be = torch.randn(96, device="cuda", generator=g)
+    _close(ops.gemm_conv(xe, we, bias=be, **conv), E.gemm_conv(cpu(xe), cpu(we), bias=cpu(be), **conv).cuda(),
+           "emulator gemm_conv end padding")
+    # row statistics of an fp32 producer (bias + residual), then a folded LayerNorm with quick-GELU reading them
+    m, k, n = 300, 320, 320
+    xa, res = _bf(torch.randn(m, k, device="cuda", generator=g)), _bf(torch.randn(m, n, device="cuda", generator=g) + 16)
+    wp, bp = _bf(torch.randn(n, k, device="cuda", generator=g) / math.sqrt(k)), torch.randn(n, device="cuda", generator=g)
+    prod = dict(n_img=1, h_in=1, w_in=m, c0=k, lda0=k, n_out=n, ldr=n, out_f32=True, emit_stats=True)
+    dx, dst_ = ops.gemm_conv(xa, wp, bias=bp, residual=res, **prod)
+    ex, est = E.gemm_conv(cpu(xa), cpu(wp), bias=cpu(bp), residual=cpu(res), **prod)
+    _close_f32(dx, ex.cuda(), "emulator gemm_conv fp32 producer")
+    stored = dx.to(F64)
+    bound = 3e-5 * torch.stack([stored.abs().sum(1), (stored * stored).sum(1)], -1)
+    _within("emulator gemm_conv row statistics", est.data.sum(1).cuda(), dst_.data.sum(1).to(F64), bound, "row statistics")
+    xb, wg = _bf(dx), _bf(torch.randn(512, n, device="cuda", generator=g) / math.sqrt(n))
+    cs, cb = wg.float().sum(1), torch.randn(512, device="cuda", generator=g)
+    cons = dict(n_img=1, h_in=1, w_in=m, c0=n, lda0=n, n_out=512, ln_eps=1e-5, quick_gelu=True)
+    _close(ops.gemm_conv(xb, wg, bias=cb, ln=dst_, ln_colsum=cs, **cons),
+           E.gemm_conv(cpu(xb), cpu(wg), bias=cpu(cb), ln=ops.RowStats(cpu(dst_.data), dst_.parts), ln_colsum=cpu(cs),
+                       **cons).cuda(), "emulator gemm_conv folded LayerNorm + quick-GELU")
+
+    # attention: an empty slot and per-batch key counts (one batch without keys); two K/V sources; causal
+    heads, d, lq, lk = 2, 64, 70, 90
+    c = heads * d
+    q = _bf(torch.randn(3 * lq, c, device="cuda", generator=g))
+    kv = _bf(torch.randn(4 * lk, 2 * c, device="cuda", generator=g))
+    kv2 = _bf(torch.randn(2 * lk, 2 * c, device="cuda", generator=g))
+    idx = torch.tensor([[0, -1], [-1, 2], [3, 1]], dtype=I32, device="cuda")
+    kv_len = torch.tensor([90, 37, 0], dtype=I32, device="cuda")
+    att = dict(b=3, heads=heads, lq=lq, lk=lk, d=d, ldq=c, scale=d ** -0.5, n_sets=2)
+    dev = ops.attention(q, kv[:, :c], kv[:, c:], b_kv=4, ldk=2 * c, ldv=2 * c, kv_index=idx, kv_len=kv_len, **att)
+    emu = E.attention(cpu(q), cpu(kv)[:, :c], cpu(kv)[:, c:], b_kv=4, ldk=2 * c, ldv=2 * c, kv_index=cpu(idx),
+                      kv_len=cpu(kv_len), **att)
+    _attn_close(dev, emu.cuda().to(F64), 2)
+    assert not dev[2 * lq:].any() and not emu[2 * lq:].any()
+    idx2 = torch.tensor([[1 << 24, 3], [2, (1 << 24) | 1], [-1, 1 << 24]], dtype=I32, device="cuda")
+    srcs = lambda t, t2: [(t[:, :c], t[:, c:], 2 * c, 4), (t2[:, :c], t2[:, c:], 2 * c, 2)]  # noqa: E731
+    dev = ops.attention_multi(q, srcs(kv, kv2), kv_index=idx2, **att)
+    _attn_close(dev, E.attention_multi(cpu(q), srcs(cpu(kv), cpu(kv2)), kv_index=cpu(idx2), **att).cuda().to(F64), 2)
+    qkv = _bf(torch.randn(2 * 77, 3 * c, device="cuda", generator=g))
+    causal = dict(b=2, heads=heads, l=77, d=d, ldq=3 * c, ldk=3 * c, ldv=3 * c, scale=d ** -0.5)
+    dev = ops.attention_causal(qkv[:, :c], qkv[:, c:2 * c], qkv[:, 2 * c:], **causal)
+    qc = cpu(qkv)
+    _attn_close(dev, E.attention_causal(qc[:, :c], qc[:, c:2 * c], qc[:, 2 * c:], **causal).cuda().to(F64))
+
+    # FID pools (max bitwise) and input step; CLIP embedding (bitwise, statistics within 3e-5 * sum|x|, sum x^2)
+    xp = _bf(torch.randn(2 * 17 * 17, 96, device="cuda", generator=g))
+    pool = dict(n=2, h=17, w=17, c=80, ldx=96)
+    for mode, k_, s_, p_ in ((ops.POOL_MAX, 3, 2, 0), (ops.POOL_AVG, 3, 1, 1), (ops.POOL_GLOBAL_AVG, 3, 1, 0)):
+        dev, emu = ops.pool2d(xp, mode=mode, k=k_, stride=s_, pad=p_, **pool), E.pool2d(cpu(xp), mode=mode, k=k_, stride=s_, pad=p_, **pool)
+        if mode == ops.POOL_MAX:
+            same(dev, emu, "pool2d max")
+        else:
+            _close(dev, emu.cuda(), f"emulator pool2d mode {mode}")
+    img = torch.rand(2, 3, 60, 90, device="cuda", generator=g)
+    dev = ops.fid_input(img, nhwc=False, quantize=True, normalize=True, size=(75, 97))
+    emu = E.fid_input(cpu(img), nhwc=False, quantize=True, normalize=True, size=(75, 97))
+    assert (dev.cpu().to(F64) - emu.to(F64)).abs().max().item() <= 2.0 ** -8 * emu.abs().max().item() + 1e-6
+    tok, pos = _bf(torch.randn(500, 768, device="cuda", generator=g)), _bf(torch.randn(77, 768, device="cuda", generator=g))
+    ids = torch.randint(0, 500, (2, 77), dtype=I32, device="cuda", generator=g)
+    ids[1, 3] = 500  # outside the vocabulary: a NaN row
+    (dx, dst_), (ex, est) = ops.clip_embed(ids, tok, pos), E.clip_embed(cpu(ids), cpu(tok), cpu(pos))
+    same(dx, ex, "clip_embed")
+    ok = ~dx.isnan().any(1)
+    stored = dx[ok].to(F64)
+    bound = 3e-5 * torch.stack([stored.abs().sum(1), (stored * stored).sum(1)], -1)
+    _within("emulator clip_embed statistics", est.data[:, 0][ok.cpu()].cuda(), dst_.data[:, 0][ok].to(F64), bound, "clip_embed")

@@ -1,7 +1,7 @@
 """AutoencoderKL.encode without a GPU: the encoder's parameter names against the reference, the fp32 oracle
 (oracle/vae_encode.py) against the reference's own encode (fixture tests/golden/vae_encode.pt, oracle/make_golden_vae_encode.py,
 and directly when the reference tree is present), the real VaeEncoderEngine / AutoencoderKL.encode / encode_latents host code
-through tests/vae_encode_emulator.py, and the loading rules of the encoder weights."""
+through tests/ops_emulator.py, and the loading rules of the encoder weights."""
 import json
 import os
 from dataclasses import asdict
@@ -9,11 +9,11 @@ from dataclasses import asdict
 import pytest
 import torch
 
-from magicdrive_b200 import arch, models
+from magicdrive_b200 import arch, engine, models
 from oracle import ref_shim
 from oracle import vae_encode as OV
 from oracle.make_golden_vae_encode import CASES, full_state_dict, images, reference_vae, vae_config
-from tests import vae_encode_emulator
+from tests import ops_emulator
 from tests.common import GOLDEN, rel_l2
 
 needs_ref = pytest.mark.skipif(not ref_shim.available(), reason="needs the reference tree (or its oracle/_ref snapshot)")
@@ -29,7 +29,8 @@ def _bf16_exact(sd):
 
 @pytest.fixture
 def emulated(monkeypatch):
-    vae_encode_emulator.install(monkeypatch)
+    ops_emulator.install(monkeypatch)
+    monkeypatch.setattr(engine._Weights, "fold_dtype", torch.float32)  # the quant_conv fold's algebra to fp32
 
 
 # ------------------------------------------------------------------------------------------------------------ shapes
@@ -132,12 +133,6 @@ def test_sd15_encoder_layout_through_emulated_operators(emulated):
     out = vae.encode(x).latent_dist.parameters
     ref = OV.vae_encode_moments(sd, cfg, x)
     assert out.shape == ref.shape == (1, 8, 3, 4) and rel_l2(out, ref) < 1e-5
-
-
-def test_emulated_gemm_conv_rejects_keywords_it_does_not_know():
-    a = torch.zeros(16, 64)
-    with pytest.raises(TypeError):
-        vae_encode_emulator.gemm_conv(a, torch.zeros(8, 64), n_img=1, h_in=4, w_in=4, c0=64, lda0=64, n_out=8, geglu=True)
 
 
 # ------------------------------------------------------------------------------------------------------------ loading
