@@ -186,7 +186,13 @@ int mdb_attention_multi(const void* q, int ldq, int n_src, const void* const* k,
  * Keys at or beyond kv_len[b] take no weight and key tiles past it are not loaded.  The kernel clamps each entry to [0, lk]
  * (a batch with 0 keys contributes nothing, like an empty slot).  This is the cross-view "concat" mode
  * (blocks.py:122-133) when views have different neighbour counts: their neighbours' tokens are gathered into
- * [b, lk, heads*d] with kv_len[b] = neighbours * tokens. */
+ * [b, lk, heads*d] with kv_len[b] = neighbours * tokens.
+ * With one set and lk <= 256 it is also the conditioning cross-attention of a denoiser whose K/V buffers are sized for a box
+ * capacity (lk = 1 + 77 + capacity, kv_len[b] = 1 + 77 + boxes of the scene, changed between replays of a captured graph):
+ * such a launch may walk several query tiles per CTA with up to a ring of key tiles (4 x 128 keys for d <= 64, 4 x 64 for
+ * d = 80, 3 x 64 for d = 160) kept in shared memory, or stream them where kv_len[b] needs more.  For every kv_len[b] the
+ * output is bitwise that of the launch with lk = kv_len[b].  Rows at or past kv_len[b] that share the last walked key tile
+ * with counted keys are loaded and weighted 0: they must hold finite values. */
 int mdb_attention_varlen(const void* q, int ldq, int n_src, const void* const* k, const int* ldk, const void* const* v,
                          const int* ldv, const int* b_kv, void* out, int ldo, int b, int heads, int lq, int lk, int d,
                          const int* kv_index, int n_sets, const int* kv_len, float scale, void* stream);

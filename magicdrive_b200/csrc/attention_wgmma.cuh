@@ -15,6 +15,10 @@
 //   that count are neither loaded nor walked (the "concat" mode with uneven neighbour counts).
 //   Multi-Q mode (p.q_step > 0): the CTA walks the query tiles blockIdx.x, blockIdx.x + q_step, ... of its (batch, head);
 //   with a single K/V tile (lk <= BN, one set: the text / camera / box cross-attention) that tile is loaded once.
+//   KVRES (multi-Q launches with kv_len, one set): the key count is only known on the device, so each CTA decides from its
+//   own batch's tile count: up to STAGES key tiles (the whole ring) are loaded once and stay resident while the CTA walks its
+//   query tiles; a batch with more tiles streams them through the ring per query tile.  Either way the tiles are walked in
+//   ascending order with the same width and the same updates, so the output is bitwise that of the lk = kv_len[b] launch.
 //   CAUSAL (self-attention with lq == lk, one set): key j is visible to query i iff j <= i.  A query tile walks only the key
 //   tiles up to the one holding its last row's diagonal (ascending, so tile 0, which holds key 0, always comes first), and
 //   producer and consumers derive that count from the same q0.
@@ -66,7 +70,7 @@ struct AttnCfg {
   static_assert(STAGES >= 1 && kSmemBytes <= 232448, "shared memory");
 };
 
-template <int D, int BN_, bool CAUSAL = false>
+template <int D, int BN_, bool CAUSAL = false, bool KVRES = false>
 __global__ void __launch_bounds__(AttnCfg<D, BN_>::kThreads, 1)
 attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ AttnKvMaps kvm, const AttnParams p) {
   using Cfg = AttnCfg<D, BN_>;
@@ -110,7 +114,8 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
   // kv_index / kv_len may be written by the predecessor kernel: read only after the PDL wait
   const int lkb = p.kv_len ? min(max(p.kv_len[b], 0), p.lk) : p.lk;  // keys of this batch; the maps never go past lk
   const int ntiles = (lkb + BN - 1) / BN;
-  const bool kv_resident = ntiles == 1 && p.n_sets == 1 && n_own > 1;
+  static_assert(!(CAUSAL && KVRES), "resident key tiles: every query tile walks all of them");
+  const bool kv_resident = (KVRES ? ntiles <= STAGES : ntiles == 1) && p.n_sets == 1 && n_own > 1;
   auto kv_entry = [&](int set) { return p.kv_index ? p.kv_index[b * p.n_sets + set] : b; };
   // key tiles the set with kv_index entry kve reads for the query tile starting at q0: none for an empty slot; causal tiles
   // stop at the one holding key min(q0 + ATT_BM, lq) - 1.  Producer and consumers both take their counts from here.
@@ -174,7 +179,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
       for (int i = 0; i < Cfg::OACC; ++i) oacc[i] = 0.f;
       float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
       for (int j = 0; j < nt; ++j) {
-        const int st = kv_resident ? 0 : stage;
+        const int st = kv_resident ? (KVRES ? j : 0) : stage;  // resident tile j sits in ring slot j
         mbar_wait(&kv_full[st], kv_resident ? 0u : phase);
         // ---- S = Q K^T
         float s[Cfg::SACC];

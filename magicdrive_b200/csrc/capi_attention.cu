@@ -5,7 +5,7 @@
 // softmax per KV batch and writes their sum (empty slots, kv_index < 0, add nothing): the cross-view "add" mode of
 // BasicMultiviewTransformerBlock (magicdrive/networks/blocks.py:112-121, 213-217) for any neighbour count up to
 // MDB_ATT_MAX_SETS.  mdb_attention_varlen also takes a per-batch key count (the "concat" mode with uneven neighbour
-// counts).  K/V may be spread over up to three
+// counts, and the conditioning cross-attention over K/V buffers sized for a box capacity).  K/V may be spread over up to three
 // buffers (mdb_attention_multi): in view-sharded runs the neighbour views' K/V are read in place from the ring-neighbour
 // GPUs' buffers through NVLink peer memory (the tensor maps simply point at peer-mapped addresses).
 // mdb_attention_causal is the CLIP text encoder's masked self-attention (one set, one source, lq == lk).
@@ -65,9 +65,10 @@ int attn_num_sms() {
 }
 
 // Query tiles per CTA walk (AttnParams::q_step) when one K/V tile covers all keys: one CTA per SM, each keeping its K/V tile
-// and walking ~nq / gx query tiles.  0 = one tile per CTA.  MDB_ATTN_MULTIQ=0 disables it.
-int multi_q_step(int b, int heads, int lq, int lk, int n_sets, int bn) {
-  if (lk > bn || n_sets != 1) return 0;
+// and walking ~nq / gx query tiles.  0 = one tile per CTA.  MDB_ATTN_MULTIQ=0 disables it.  `resident` (the KVRES kernel):
+// the key count is a device value and the kernel keeps up to a ring of key tiles, so lk does not decide here.
+int multi_q_step(int b, int heads, int lq, int lk, int n_sets, int bn, bool resident) {
+  if ((lk > bn && !resident) || n_sets != 1) return 0;
   const char* e = getenv("MDB_ATTN_MULTIQ");
   if (e && e[0] == '0') return 0;
   const int nq = (lq + mdb::ATT_BM - 1) / mdb::ATT_BM;
@@ -80,13 +81,21 @@ int multi_q_step(int b, int heads, int lq, int lk, int n_sets, int bn) {
   return static_cast<int>(gx);
 }
 
-template <int D, int BN_, bool CAUSAL>
+// One set with a device key count over at most this many keys (the conditioning cross-attention of a denoiser with a box
+// capacity: camera + 77 text tokens + up to 178 boxes) takes the KVRES kernel: multi-Q with the key tiles resident.
+constexpr int ATT_RESIDENT_MAX_LK = 256;
+
+template <int D, int BN_, bool CAUSAL, bool KVRES = false>
 int launch_attention(const void* q, int ldq, const KvSources& src, void* out, int ldo, int b, int heads, int lq, int lk,
                      const int* kv_index, int n_sets, const int* kv_len, float scale, cudaStream_t st) {
   using Cfg = mdb::AttnCfg<D, BN_>;
+  if constexpr (!CAUSAL && !KVRES) {
+    if (kv_len && n_sets == 1 && lk <= ATT_RESIDENT_MAX_LK)
+      return launch_attention<D, BN_, false, true>(q, ldq, src, out, ldo, b, heads, lq, lk, kv_index, n_sets, kv_len, scale, st);
+  }
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(mdb::attention_wgmma_kernel<D, BN_, CAUSAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(mdb::attention_wgmma_kernel<D, BN_, CAUSAL, KVRES>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e != cudaSuccess) return mdb::set_error(MDB_ERR_CUDA, "attention_wgmma_kernel smem attr: %s", cudaGetErrorString(e));
     attr = true;
   }
@@ -98,9 +107,9 @@ int launch_attention(const void* q, int ldq, const KvSources& src, void* out, in
   p.out = static_cast<__nv_bfloat16*>(out);
   p.ldo = ldo, p.lq = lq, p.lk = lk, p.kv_index = kv_index, p.n_sets = n_sets, p.kv_len = kv_len, p.n_src = src.n;
   p.scale_log2 = scale * 1.4426950408889634f;
-  p.q_step = multi_q_step(b, heads, lq, lk, n_sets, Cfg::BN);
+  p.q_step = multi_q_step(b, heads, lq, lk, n_sets, Cfg::BN, KVRES);
   dim3 grid(p.q_step > 0 ? p.q_step : (lq + mdb::ATT_BM - 1) / mdb::ATT_BM, heads, b);
-  cudaError_t le = mdb::launch_pdl(mdb::attention_wgmma_kernel<D, BN_, CAUSAL>, grid, dim3(Cfg::kThreads), Cfg::kSmemBytes, st, tq, kvm, p);
+  cudaError_t le = mdb::launch_pdl(mdb::attention_wgmma_kernel<D, BN_, CAUSAL, KVRES>, grid, dim3(Cfg::kThreads), Cfg::kSmemBytes, st, tq, kvm, p);
   if (le != cudaSuccess) return mdb::set_error(MDB_ERR_CUDA, "attention_wgmma_kernel launch: %s", cudaGetErrorString(le));
   cudaError_t e2 = cudaGetLastError();
   if (e2 != cudaSuccess) return mdb::set_error(MDB_ERR_CUDA, "attention_wgmma_kernel: %s", cudaGetErrorString(e2));

@@ -156,6 +156,21 @@ class _Weights:
         return self.t[k]
 
 
+class CtxLen(int):
+    """Rows per view-sample of the conditioning K/V buffers, an int wherever `lc` is passed, that also carries `kv_len`: an
+    int32 [V] device tensor of the rows each view-sample attends to (1 camera + text + present boxes).  The buffers are
+    then sized once for a box capacity and the count is read by the attention kernel, so it can change between replays of
+    a captured graph (pipeline.BEVControlNetDenoiser(box_capacity=))."""
+
+    def __new__(cls, rows: int, kv_len: torch.Tensor):
+        self = super().__new__(cls, rows)
+        self.kv_len = kv_len
+        return self
+
+    def views(self, sl: slice) -> "CtxLen":
+        return CtxLen(int(self), self.kv_len[sl])
+
+
 class _Net:
     """Shared machinery of the UNet and the ControlNet encoder."""
 
@@ -264,6 +279,8 @@ class _Net:
 
     def set_view_shard(self, shard) -> None:
         """Split the cameras across ranks (dist.ShardContext) or back to all views on this GPU (None)."""
+        if shard is self.view_shard:
+            return  # unchanged: the index tensors may be held by another denoiser's captured graph, keep them alive
         self.view_shard = shard
         self._kv_idx = {}
         self._kv_sym = {}
@@ -326,7 +343,10 @@ class _Net:
         wq, cq, sq = W.ln_lin(blk + ".attn2.lnq", blk + ".norm2", [blk + ".attn2.to_q"])
         q = ops.linear(X, wq, bias=cq, ln=sx, ln_colsum=sq)
         kv = ctx_kv[p]
-        o = ops.attention(q, kv, kv[:, C:], b=V, heads=heads, lq=L, lk=lc, d=d, ldq=C, ldk=2 * C, ldv=2 * C, scale=scale)
+        # a CtxLen with a device key count (a denoiser with a box capacity): keys past kv_len[view] are not attended
+        counted = {} if getattr(lc, "kv_len", None) is None else {"kv_len": lc.kv_len}
+        o = ops.attention(q, kv, kv[:, C:], b=V, heads=heads, lq=L, lk=int(lc), d=d, ldq=C, ldk=2 * C, ldv=2 * C, scale=scale,
+                          **counted)
         wo, bo = W.lin(blk + ".attn2.to_out.0")
         X, sx = ops.linear(o, wo, bias=bo, residual=X, emit_stats=True)
         # --- cross-view attention

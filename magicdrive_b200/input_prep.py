@@ -21,11 +21,18 @@ def _t(x, dtype):
     return (torch.from_numpy(x) if isinstance(x, np.ndarray) else x).to(dtype)
 
 
-def collate_on_device(examples: List[Dict], device, max_len: Optional[int] = None, stream=None) -> Dict:
+def collate_on_device(examples: List[Dict], device, max_len: Optional[int] = None, stream=None,
+                      capacity: Optional[int] = None) -> Dict:
     """-> dict(camera_param (B, V, 3, 7) fp32, bev_map_with_aux (B, C, H, W) fp32, kwargs={"bboxes_3d_data": dict | None}) on
     `device`, the same values `collate_fn(..., bbox_mode="all-xyz", bbox_view_shared=False)` produces.
     max_len=None pads the boxes to the longest visible list of the batch like the reference (needs one device -> host read
-    of the per-view counts); an int fixes the capacity (`bbox_max_length` semantics) and stays asynchronous."""
+    of the per-view counts); an int fixes the capacity (`bbox_max_length` semantics) and stays asynchronous.
+    capacity=N (instead of max_len) is the reference's padding without that read: the tensors have N slots per view, the
+    first `count` of them are what max_len=None returns, and `count`, an int32 device scalar holding the batch's longest
+    visible list, comes back as bboxes_3d_data["count"] for a BEVControlNetDenoiser(box_capacity=N) to attend by.  Lists
+    longer than N are cut at N (`counts` holds the uncut per-view numbers)."""
+    if capacity is not None and max_len is not None:
+        raise ValueError("pass max_len or capacity, not both")
     dev = torch.device(device)
     if dev.type != "cuda":
         raise _lib.MdbError("collate_on_device runs on a CUDA device; there is no CPU fallback")
@@ -50,7 +57,7 @@ def collate_on_device(examples: List[Dict], device, max_len: Optional[int] = Non
     ret = {"camera_param": cam, "bev_map_with_aux": d(bev), "kwargs": {"bboxes_3d_data": None}}
     if sum(counts) == 0:
         return ret
-    cap = max(counts) if max_len is None else int(max_len)
+    cap = int(capacity) if capacity is not None else max(counts) if max_len is None else int(max_len)
     ob = torch.empty((B, V, cap, 8, 3), dtype=F32, device=dev)
     oc = torch.empty((B, V, cap), dtype=torch.int64, device=dev)
     om = torch.empty((B, V, cap), dtype=torch.uint8, device=dev)
@@ -58,6 +65,10 @@ def collate_on_device(examples: List[Dict], device, max_len: Optional[int] = Non
     check(L.mdb_prepare_boxes(boxes_d.data_ptr(), box_dim, labels_d.data_ptr(), off_d.data_ptr(), B, l2c_d.data_ptr(),
                               aug_d.data_ptr(), V, cap, ob.data_ptr(), oc.data_ptr(), om.data_ptr(), cnt.data_ptr(), st),
           "mdb_prepare_boxes")
+    if capacity is not None:
+        ret["kwargs"]["bboxes_3d_data"] = {"bboxes": ob, "classes": oc, "masks": om.bool(), "counts": cnt,
+                                           "count": cnt.max().clamp(max=cap).to(torch.int32)}
+        return ret
     if max_len is None:
         longest = int(cnt.max().item())  # the reference sizes the padding by the batch's longest visible list (utils.py:222-239)
         if longest == 0:

@@ -19,7 +19,7 @@ import os
 import torch
 
 from . import ops
-from .engine import FMap
+from .engine import CtxLen, FMap
 from .models import BEVControlNetModel, UNet2DConditionModelMultiview
 
 F32, BF16 = torch.float32, torch.bfloat16
@@ -141,18 +141,27 @@ class BEVControlNetDenoiser:
 
     def __init__(self, unet: UNet2DConditionModelMultiview, controlnet: BEVControlNetModel, use_cuda_graph: bool = True,
                  overlap_controlnet: bool = True, view_shard=None, scheduler: str = "ddim", vae=None,
-                 cfg_streams: bool = False, text_encoder=None, tokenizer=None):
+                 cfg_streams: bool = False, text_encoder=None, tokenizer=None, box_capacity: Optional[int] = None):
         """view_shard: a dist.ShardContext to spread each scene's guidance halves x camera views over the ranks of the job
         (inputs are still passed in full on every rank; the result is gathered back to (S, n_cam, ...)).
         scheduler: "ddim" (eta = 0) or "unipc" (the reference's default sampler, misc/test_utils.py:129).
         vae: a models.AutoencoderKL; enables output_type "pt" / "np" (decode_latents, pipeline_bev_controlnet.py:100-112).
         text_encoder / tokenizer: a models.CLIPTextModel and a transformers CLIPTokenizer; enable `prompt=` /
         `negative_prompt=` captions in place of precomputed embeddings (_encode_prompt, pipeline_controlnet.py:285-430).
+        box_capacity: None keeps one resident state (and one pair of CUDA graphs) per box count.  An int N sizes the box
+        inputs, the context and its K/V buffers once for N boxes per view and keeps the number actually attended in device
+        memory (st["ctx_len"]): calls with any n <= N boxes then refresh the same state and replay the same graphs, with the
+        result of the exact-shape call (the stream of scenes of a data-set run, `generate_stream`).
         cfg_streams (opt-in, not yet measured): run the unconditional and the conditional half of the guidance batch as
         two concurrent branches (ControlNet -> UNet each) instead of ControlNet || UNet-encoder on the whole batch, so
         every kernel's fixed cost is overlapped by the other half's kernels; same arithmetic per sample."""
         if scheduler not in ("ddim", "unipc"):
             raise ValueError(f"scheduler must be 'ddim' or 'unipc', got {scheduler!r}")
+        if box_capacity is not None and (int(box_capacity) != box_capacity or box_capacity < 1):
+            raise ValueError(f"box_capacity must be a positive int or None, got {box_capacity!r}")
+        if box_capacity is not None and view_shard is not None:
+            raise ValueError("box_capacity is not implemented for view-sharded runs (view_shard=)")
+        self.box_capacity = None if box_capacity is None else int(box_capacity)
         self.unet, self.controlnet, self.vae = unet, controlnet, vae
         self.text_encoder, self.tokenizer = text_encoder, tokenizer
         self.overlap_controlnet = overlap_controlnet
@@ -252,11 +261,12 @@ class BEVControlNetDenoiser:
             views = slice(half * vh, (half + 1) * vh)
             c_kv = {k: v[rows] for k, v in st["c_kv"].items()}
             u_kv = {k: v[rows] for k, v in st["u_kv"].items()}
+            lc_h = lc.views(views) if isinstance(lc, CtxLen) else lc
 
             def branch():
-                down, mid, _, _ = ce.forward(x, vh, h, w, st["t_dev"][views], c_kv, lc, st["map"][views], st["cond_scale"],
+                down, mid, _, _ = ce.forward(x, vh, h, w, st["t_dev"][views], c_kv, lc_h, st["map"][views], st["cond_scale"],
                                              temb_all=st["c_temb"])
-                e = ue.forward(x, vh, h, w, st["t_dev"][views], u_kv, lc, down, mid, temb_all=st["u_temb"])
+                e = ue.forward(x, vh, h, w, st["t_dev"][views], u_kv, lc_h, down, mid, temb_all=st["u_temb"])
                 eps[half * npix:(half + 1) * npix].copy_(e)
             if on_gpu and half == 1:
                 with torch.cuda.stream(side), ops.workspace_slot(1):
@@ -359,12 +369,16 @@ class BEVControlNetDenoiser:
         prompt_embeds = prompt_embeds.to(F32)
         image = image.to(F32)
         boxes = bboxes_3d_data
+        # with a box capacity the attended number of boxes may come as a device scalar (collate_on_device(capacity=))
+        cap = self.box_capacity
+        count = None if cap is None or boxes is None else boxes.get("count")
         if cfg:
             # unconditional half of the BEV map: the scene's map, zeros on request (:296-300), or the ControlNet's
             # configured uncond map (add_uncond_to_kwargs -> substitute_with_uncond_map)
             uncond_image = torch.zeros_like(image) if use_zero_map_as_unconditional else image
+            # boxes that carry a device count are already at capacity: bbox_max_length then only raises the attended count
             kw = cn.add_uncond_to_kwargs(camera_param=camera_param, bboxes_3d_data=boxes, image=uncond_image,
-                                         max_len=bbox_max_length)
+                                         max_len=None if count is not None else bbox_max_length)
             camera_param, boxes = kw["camera_param"], kw["bboxes_3d_data"]
             text = torch.cat([negative_prompt_embeds.to(prompt_embeds), prompt_embeds])
             image = torch.cat([kw["image"].to(image), image])
@@ -384,6 +398,25 @@ class BEVControlNetDenoiser:
         S_, _, c, h, w = lat.shape
         lat_nhwc = lat.reshape(S * n_cam, c, h, w).permute(0, 2, 3, 1).contiguous().view(-1, c)
         V = S * n_cam * dup
+        n_boxes = 0 if boxes is None else boxes["bboxes"].shape[2]
+        if cap is not None:
+            # stage the boxes at capacity (rows past n: zero boxes, class 0, mask false; never attended) and keep the
+            # attended number apart: an int, or the device scalar a collate at capacity returns (no host round trip)
+            if n_boxes > cap:
+                raise ValueError(f"{n_boxes} boxes per view exceed box_capacity={cap}")
+            if count is not None and cfg and bbox_max_length is not None:
+                if bbox_max_length > cap:
+                    raise ValueError(f"bbox_max_length={bbox_max_length} exceeds box_capacity={cap}")
+                count = count.clamp(min=bbox_max_length)
+            lead = (camera_param.shape[0], n_cam)
+            box_dev = camera_param.device if boxes is None else boxes["bboxes"].device
+            padded = dict(bboxes=torch.zeros(*lead, cap, 8, 3, dtype=F32, device=box_dev),
+                          classes=torch.zeros(*lead, cap, dtype=torch.long, device=box_dev),
+                          masks=torch.zeros(*lead, cap, dtype=torch.bool, device=box_dev))
+            if boxes is not None:
+                for k, v in padded.items():
+                    v[:, :, :n_boxes] = boxes[k]
+            boxes = padded
         lc = 1 + text.shape[1] + (0 if boxes is None else boxes["bboxes"].shape[2])
         pin_mode, pin_mask, pin_cond = None, None, None
         if conditional_latents is not None and any(c is not None for row in conditional_latents for c in row):
@@ -413,6 +446,8 @@ class BEVControlNetDenoiser:
             if pin_mode is not None:
                 st["pin"]["noise0"].copy_(st["inputs"]["latents"])
             st["guidance"], st["cond_scale"] = float(guidance_scale), float(controlnet_conditioning_scale)
+            if cap is not None:
+                self._set_ctx_len(st, 1 + text.shape[1], n_boxes, count)
             if self.use_cuda_graph and st["inputs"]["latents"].is_cuda:
                 if self._cond_graph is None or self._cond_graph_state is not st:
                     torch.cuda.synchronize()
@@ -434,9 +469,22 @@ class BEVControlNetDenoiser:
                   pin=None if pin_mode is None else dict(
                       mode=pin_mode, mask=dev_in["pin_mask"], cond=dev_in["pin_cond"], noise0=dev_in["latents"].clone(),
                       coef_dev=torch.zeros(2, dtype=F32, device=dev), one=torch.tensor([0.0, 1.0], dtype=F32, device=dev)))
+        if cap is not None:
+            st["ctx_len"] = torch.zeros(V, dtype=torch.int32, device=dev)
+            st["lc"] = CtxLen(lc, st["ctx_len"])
+            self._set_ctx_len(st, 1 + text.shape[1], n_boxes, count)
         self._encode_conditions(st)
         self._static, self._graph, self._cond_graph = st, None, None
         return st
+
+    @staticmethod
+    def _set_ctx_len(st, lead: int, n_boxes: int, count):
+        """st["ctx_len"][:] = camera + text tokens + attended boxes, in place (the captured graphs read it from memory)."""
+        if count is None:
+            st["ctx_len"].fill_(lead + n_boxes)
+        else:
+            st["ctx_len"].copy_(count.to(torch.int32).clamp(max=n_boxes).reshape(1).expand_as(st["ctx_len"]), non_blocking=True)
+            st["ctx_len"].add_(lead)
 
     def _encode_conditions(self, st):
         """Everything that depends on the conditioning but not on the latents or the timestep, from the resident input
@@ -581,12 +629,51 @@ class BEVControlNetDenoiser:
                           use_zero_map_as_unconditional, bbox_max_length,
                           latent_hw=((height or ss) // 8, (width or ss) // 8))
         ts = self.set_schedule(st, num_inference_steps)
-        self.run_steps(st, 0, len(ts))  # UniPC drops duplicate rounded timesteps: run what the schedule holds
+        return self._sample(st, len(ts), output_type)
+
+    def _sample(self, st, n_steps, output_type):
+        self.run_steps(st, 0, n_steps)  # UniPC drops duplicate rounded timesteps: run what the schedule holds
         latents = self.latents_out(st)
         if output_type == "latent":
             return latents
         images = self.vae.decode_latents(latents)  # (S, n_cam, H, W, 3) in [0, 1]
         return images.cpu().numpy() if output_type == "np" else images
+
+    @torch.no_grad()
+    def generate_stream(self, batches, *, samples_per_scene: int = 1, generator: Optional[torch.Generator] = None,
+                        **call_kwargs):
+        """The reference's data-set loop (run_one_batch_pipe, misc/test_utils.py:191-255) over an iterable of collated
+        batches: dicts with `image` (or `bev_map_with_aux`), `camera_param`, `prompt` or `prompt_embeds` (and optionally
+        `negative_prompt` / `negative_prompt_embeds`) and `kwargs` (bev_controlnet_kwargs).  Yields per batch the list of
+        its `samples_per_scene` results, each what one call with `call_kwargs` returns.  The samples of a batch differ
+        only in their initial noise, drawn from the one `generator` in call order exactly as repeated calls would draw it, so
+        after the first sample nothing is staged or encoded again: the latents are re-drawn into the resident state and the
+        steps run.  With `box_capacity` the batches may hold any number of boxes and all replay the same graphs."""
+        if samples_per_scene < 1:
+            raise ValueError("samples_per_scene must be at least 1")
+        if "latents" in call_kwargs:
+            raise ValueError("generate_stream draws the initial noise itself; pass generator=")
+        output_type = call_kwargs.get("output_type", "latent")
+        for batch in batches:
+            named = {k: batch[k] for k in ("prompt", "prompt_embeds", "negative_prompt", "negative_prompt_embeds") if k in batch}
+            image = batch["image"] if "image" in batch else batch["bev_map_with_aux"]
+            results = [self(image, batch["camera_param"], bev_controlnet_kwargs=batch.get("kwargs"), generator=generator,
+                            **named, **call_kwargs)]
+            st = self._static
+            n_steps = len(self.scheduler.timesteps)
+            c, (h, w) = st["latents"].shape[1], (st["h"], st["w"])
+            for _ in range(samples_per_scene - 1):
+                if self.view_shard is not None:  # each rank holds a slice of the views: stage through the full call
+                    results.append(self(image, batch["camera_param"], bev_controlnet_kwargs=batch.get("kwargs"),
+                                        generator=generator, **named, **call_kwargs))
+                    continue
+                noise = torch.randn(st["S"], c, h, w, generator=generator)  # prepare_latents: shared by a scene's views
+                noise = torch.stack([noise] * st["n_cam"], dim=1).reshape(-1, c, h, w).permute(0, 2, 3, 1)
+                st["latents"].copy_(noise.reshape(-1, c))
+                if st["pin"] is not None:
+                    st["pin"]["noise0"].copy_(st["latents"])
+                results.append(self._sample(st, n_steps, output_type))
+            yield results
 
     def latents_out(self, st):
         S, n_cam, h, w = st["S"], st["n_cam"], st["h"], st["w"]
