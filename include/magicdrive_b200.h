@@ -135,6 +135,27 @@ int mdb_pool2d(const void* x, int ldx, int n, int h, int w, int c, int mode, int
 int mdb_fid_input(const void* x, int x_is_f32, int x_is_nhwc, int n, int h, int w, int quantize, int normalize, void* out,
                   int ho, int wo, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * FID evaluation protocol (perception/data_prepare/val_set_gen.py:29-43, 103-116; tools/fid_score.py:361-368, 474-482):
+ * the 8-bit steps between the pipeline's views and Inception, equal byte for byte to Pillow's.
+ * mdb_resample_u8: Pillow's bicubic resample (Image.resize(..., BICUBIC), a = -0.5, support widened by the scale when
+ *   downsampling) of n images h x w -> rh x rw, RGB.  x: uint8 NHWC, or (x_is_f32) fp32 [0, 1] NHWC / NCHW rounded to
+ *   uint8 first as (x * 255).round() (diffusers numpy_to_pil).  coef_w / coef_h: int32 [rw, taps_w + 2] / [rh, taps_h + 2],
+ *   row i = [first input index, tap count, 22-bit fixed-point weights...]; a pass is run exactly when its size changes and
+ *   its coefficients must then be given (NULL otherwise).  The horizontal pass runs first and is rounded and clipped to
+ *   uint8 (tmp: uint8 [n, h, crop_w, 3], needed when the width changes).  Of the resized image, the window rows
+ *   [crop_top, crop_top + crop_h) x columns [crop_left, crop_left + crop_w) is written at (top, left) of out, uint8 NHWC
+ *   [n, out_h, out_w, 3]; every other out pixel is 0 (a zero pad).
+ * mdb_jpeg_roundtrip_u8: uint8 NHWC RGB [n, h, w, 3] -> the image a baseline JPEG at `quality` (1..100, the standard
+ *   tables scaled as IJG libjpeg does) with 4:2:0 chroma decodes to, as Pillow saves and loads it by default (quality 75):
+ *   integer DCTs, triangle chroma upsampling.  The entropy coder is lossless and is skipped.  planes: 8-byte aligned
+ *   scratch of n * hp * wp * 3 / 2 bytes (hp, wp: h, w rounded up to 16).  out may be x.
+ * ------------------------------------------------------------------------------------------------ */
+int mdb_resample_u8(const void* x, int x_is_f32, int x_is_nhwc, int n, int h, int w, const int* coef_w, int taps_w,
+                    int rw, const int* coef_h, int taps_h, int rh, int crop_top, int crop_left, int crop_h, int crop_w,
+                    void* tmp, void* out, int out_h, int out_w, int top, int left, void* stream);
+int mdb_jpeg_roundtrip_u8(const void* x, int n, int h, int w, int quality, void* planes, void* out, void* stream);
+
 /* Direct (CUDA-core) convolution for tiny channel counts: conv_in 4->320 (unet_2d_condition.py:231),
  * conv_out 320->4 (:503), BEV map encoder (magicdrive/networks/map_embedder.py:66-76).
  * x: [n, h, w, cin] bf16 or fp32; w: fp32 [kh, kw, cin, cout] (output channel innermost: coalesced across a warp);

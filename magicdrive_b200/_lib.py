@@ -74,6 +74,9 @@ SIGNATURES = {
     "mdb_cfg_unipc_step": (_i, [_vp, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _ll, _vp]),
     "mdb_pool2d": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),
     "mdb_fid_input": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _vp]),
+    "mdb_resample_u8": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _i,
+                             _vp]),
+    "mdb_jpeg_roundtrip_u8": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp]),
 }
 
 
