@@ -278,36 +278,56 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
       continue;
     }
     float st_s[2] = {0.f, 0.f}, st_ss[2] = {0.f, 0.f};
+    // The residual may be the output buffer itself, so a residual load cannot move above an earlier output store: loaded
+    // one element at a time, every element would wait out its own round trip to L2.  Each batch of RES_J 8-column groups
+    // loads all its residual pairs first (the thread reads only the elements it then overwrites), so one round trip
+    // serves the whole batch.
+    constexpr int RES_J = BLOCK_N == 256 ? 1 : 4;  // 256 columns of accumulators leave no registers for more
 #pragma unroll
-    for (int j = 0; j < BLOCK_N / 8; ++j) {
-      const int col = n0 + 8 * j + 2 * q;
-      if (col >= p.n_out) continue;
-      const float2 b = p.bias ? ldg_f2(p.bias + col) : make_float2(0.f, 0.f);
-      const float2 cs = has_ln ? ldg_f2(p.ln_colsum + col) : make_float2(0.f, 0.f);
+    for (int jb = 0; jb < BLOCK_N / 8; jb += RES_J) {
+      __nv_bfloat162 res[RES_J][2];
+      if (p.residual) {
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        if (!ok[h]) continue;
-        float2 cb = b;
-        if (p.rowbias) {
-          const float2 rb = ldg_f2(p.rowbias + static_cast<long long>(img[h]) * p.rowbias_ld + col);
-          cb.x += rb.x, cb.y += rb.y;
+        for (int jj = 0; jj < RES_J; ++jj) {
+          const int col = n0 + 8 * (jb + jj) + 2 * q;
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            if (col < p.n_out && ok[h])
+              res[jj][h] = *reinterpret_cast<const __nv_bfloat162*>(p.residual + pix[h] * p.ldr + col);
         }
-        float v0 = fmaf(rowA[h], acc[4 * j + 2 * h], fmaf(rowB[h], cs.x, cb.x * scale));
-        float v1 = fmaf(rowA[h], acc[4 * j + 2 * h + 1], fmaf(rowB[h], cs.y, cb.y * scale));
-        if (p.residual) {
-          const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.residual + pix[h] * p.ldr + col));
-          v0 += r.x, v1 += r.y;
+      }
+#pragma unroll
+      for (int jj = 0; jj < RES_J; ++jj) {
+        const int j = jb + jj;
+        const int col = n0 + 8 * j + 2 * q;
+        if (col >= p.n_out) continue;
+        const float2 b = p.bias ? ldg_f2(p.bias + col) : make_float2(0.f, 0.f);
+        const float2 cs = has_ln ? ldg_f2(p.ln_colsum + col) : make_float2(0.f, 0.f);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!ok[h]) continue;
+          float2 cb = b;
+          if (p.rowbias) {
+            const float2 rb = ldg_f2(p.rowbias + static_cast<long long>(img[h]) * p.rowbias_ld + col);
+            cb.x += rb.x, cb.y += rb.y;
+          }
+          float v0 = fmaf(rowA[h], acc[4 * j + 2 * h], fmaf(rowB[h], cs.x, cb.x * scale));
+          float v1 = fmaf(rowA[h], acc[4 * j + 2 * h + 1], fmaf(rowB[h], cs.y, cb.y * scale));
+          if (p.residual) {
+            const float2 r = __bfloat1622float2(res[jj][h]);
+            v0 += r.x, v1 += r.y;
+          }
+          if (p.out_is_f32) {
+            *reinterpret_cast<float2*>(static_cast<float*>(p.out) + pix[h] * p.ldo + col) = make_float2(v0, v1);
+          } else {
+            const uint32_t pk = pack_bf16(v0, v1);
+            *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.out) + pix[h] * p.ldo + col) = pk;
+            // the row statistics describe the values as stored: the consumer's folded LayerNorm multiplies these
+            v0 = __uint_as_float(pk << 16), v1 = __uint_as_float(pk & 0xffff0000u);
+          }
+          st_s[h] += v0 + v1;
+          st_ss[h] = fmaf(v0, v0, fmaf(v1, v1, st_ss[h]));
         }
-        if (p.out_is_f32) {
-          *reinterpret_cast<float2*>(static_cast<float*>(p.out) + pix[h] * p.ldo + col) = make_float2(v0, v1);
-        } else {
-          const uint32_t pk = pack_bf16(v0, v1);
-          *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.out) + pix[h] * p.ldo + col) = pk;
-          // the row statistics describe the values as stored: the consumer's folded LayerNorm multiplies these
-          v0 = __uint_as_float(pk << 16), v1 = __uint_as_float(pk & 0xffff0000u);
-        }
-        st_s[h] += v0 + v1;
-        st_ss[h] = fmaf(v0, v0, fmaf(v1, v1, st_ss[h]));
       }
     }
     if (p.stats_out != nullptr) {
