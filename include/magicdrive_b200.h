@@ -4,7 +4,9 @@
  * Every entry point takes raw device pointers, sizes, strides and a cudaStream_t (as void*), returns 0 on
  * success or a negative status, and never allocates, synchronises or takes ownership.  mdb_last_error()
  * returns a thread-local message for the last failure.  Activations are bf16, channel-innermost (NHWC for
- * feature maps == [tokens, channels] for transformer blocks); accumulation is fp32.
+ * feature maps == [tokens, channels] for transformer blocks); accumulation is fp32.  Models with fp16 parameters run
+ * the denoising step in f16: mdb_gemm_desc.operand_dtype and the *_f16 entry points below, each the f16 twin of the bf16
+ * entry point it follows, with the same signature and checks.
  *
  * The reference has no native boundary of its own for this path except one op: xformers'
  * efficient_attention_forward_cutlass (third_party/xformers/xformers/csrc/attention/attention.cpp:27,
@@ -103,6 +105,10 @@ typedef struct {
    * bf16 outputs), or NULL. */
   float* stats_out;
   int pad_h_end, pad_w_end;  /* extra zero rows below / columns right of the image (see above); 0 = symmetric padding */
+  /* Element type of a0, a1, w, residual and a non-fp32 out: 0 = bf16 (every field above says bf16), 1 = f16 (models with
+   * fp16 parameters).  f16 launches take the linear and GEGLU epilogues, split-K included, on single CTAs; quick-GELU,
+   * ReLU and kernel_variant 3 are MDB_ERR_UNSUPPORTED.  Row statistics are then taken from the f16-rounded values. */
+  int operand_dtype;
 } mdb_gemm_desc;
 
 int mdb_gemm_conv(const mdb_gemm_desc* d, void* stream);
@@ -170,6 +176,10 @@ int mdb_conv_direct(const void* x, int x_is_f32, int n, int h, int w, int cin, c
 int mdb_groupnorm(const void* x0, int c0, int ld0, const void* x1, int c1, int ld1, int n_img, int hw, int groups,
                   float eps, const float* gamma, const float* beta, int silu, void* out, int ldo, float* stats_ws,
                   void* stream);
+/* The same over f16 sources and output (fp32 statistics). */
+int mdb_groupnorm_f16(const void* x0, int c0, int ld0, const void* x1, int c1, int ld1, int n_img, int hw, int groups,
+                      float eps, const float* gamma, const float* beta, int silu, void* out, int ldo, float* stats_ws,
+                      void* stream);
 
 /* LayerNorm over the last dim of [rows, C] bf16 (attention.py:85,104,120; blocks.py:67-71). */
 int mdb_layernorm(const void* x, long long rows, int c, int ldx, const float* gamma, const float* beta, float eps,
@@ -217,6 +227,11 @@ int mdb_attention_multi(const void* q, int ldq, int n_src, const void* const* k,
 int mdb_attention_varlen(const void* q, int ldq, int n_src, const void* const* k, const int* ldk, const void* const* v,
                          const int* ldv, const int* b_kv, void* out, int ldo, int b, int heads, int lq, int lk, int d,
                          const int* kv_index, int n_sets, const int* kv_len, float scale, void* stream);
+/* The same with f16 q, k, v and output (kv_len may be NULL): P is packed to f16 for the P V product and each set's output
+ * is rounded to f16 before the sum.  One key-tile width (the default of MDB_ATTN_KERNEL); the same head dims. */
+int mdb_attention_varlen_f16(const void* q, int ldq, int n_src, const void* const* k, const int* ldk, const void* const* v,
+                             const int* ldv, const int* b_kv, void* out, int ldo, int b, int heads, int lq, int lk, int d,
+                             const int* kv_index, int n_sets, const int* kv_len, float scale, void* stream);
 
 /* Causal self-attention of the CLIP text encoder (transformers models/clip/modeling_clip.py CLIPAttention.forward with the
  * causal_attention_mask of CLIPTextTransformer.forward): as mdb_attention with one set, b_kv == b and no kv_index, and key j
@@ -235,8 +250,11 @@ int mdb_clip_embed(const void* ids, int ids_are_i64, int n_seq, int len, const v
 
 /* out = a + b (bf16), n elements (unet_2d_condition_multiview.py:464-473, 487-488). */
 int mdb_add(const void* a, const void* b, void* out, long long n, void* stream);
+/* out = a + b (f16), the sum taken in fp32 and rounded once. */
+int mdb_add_f16(const void* a, const void* b, void* out, long long n, void* stream);
 
-/* Nearest-neighbour resize NHWC, src index = floor(dst * in / out) (resnet.py:156-159). */
+/* Nearest-neighbour resize NHWC, src index = floor(dst * in / out) (resnet.py:156-159).  A copy of 2-byte elements:
+ * bf16 and f16 maps alike. */
 int mdb_upsample_nearest(const void* x, int n, int h, int w, int c, void* out, int ho, int wo, void* stream);
 /* nn.AdaptiveAvgPool2d((ho, wo)) over an NHWC fp32 map, optionally followed by SiLU: the pooling block of
  * BEVControlNetConditioningEmbeddingPlus (magicdrive/networks/map_embedder.py:118, forward :66-76 applies SiLU after every
@@ -248,6 +266,9 @@ int mdb_adaptive_avgpool(const float* x, int n, int h, int w, int c, float* out,
  * post_silu to the output (embeddings.py:192-201; resnet.py:615-616; bbox_embedder.py:145-152). */
 int mdb_linear_small(const float* in, int m, int k, int ldi, const void* w, int ldw, const float* bias, int n,
                      int pre_silu, int post_silu, float* out, int ldo, void* stream);
+/* The same with f16 weights (the time-embedding MLP and camera / box encoders of fp16 models). */
+int mdb_linear_small_f16(const float* in, int m, int k, int ldi, const void* w, int ldw, const float* bias, int n,
+                         int pre_silu, int post_silu, float* out, int ldo, void* stream);
 
 /* Sinusoidal timestep embedding, flip_sin_to_cos, freq_shift (embeddings.py:24-64).  t: fp32 [m] on device. */
 int mdb_timestep_embedding(const float* t, int m, int dim, int flip_sin_to_cos, float freq_shift, float* out,
@@ -262,11 +283,16 @@ int mdb_nchw_to_nhwc(const void* x, int x_is_f32, int n, int c, int h, int w, vo
 int mdb_nhwc_to_nchw(const void* x_bf16, int n, int c, int h, int w, void* out, int out_is_f32, void* stream);
 int mdb_f32_to_bf16(const float* x, void* out, long long n, void* stream);
 int mdb_bf16_to_f32(const void* x, float* out, long long n, void* stream);
+/* fp32 -> f16 (round to nearest even; overflow to inf) and f16 -> fp32 (exact). */
+int mdb_f32_to_f16(const float* x, void* out, long long n, void* stream);
+int mdb_f16_to_f32(const void* x, float* out, long long n, void* stream);
 
 /* Latents [pix, cin] (fp32 or bf16) -> bf16 [repeat*pix, cpad] with channels >= cin zeroed: the K-padded A operand
  * that lets conv_in (unet_2d_condition.py:231, 4 -> 320 channels) run on the tensor-core path; repeat = 2 duplicates
  * the batch for classifier-free guidance (pipeline_bev_controlnet.py:352-354). */
 int mdb_pack_latents(const void* x, int x_is_f32, long long pix, int cin, int cpad, int repeat, void* out, void* stream);
+/* The same with an f16 output; x is fp32, or f16 when x_is_f32 == 0. */
+int mdb_pack_latents_f16(const void* x, int x_is_f32, long long pix, int cin, int cpad, int repeat, void* out, void* stream);
 
 /* Classifier-free guidance + DDIM (eta = 0) update fused (pipeline_bev_controlnet.py:426-436;
  * scheduling_ddim.py:325-445).  eps: fp32 [(2 if cfg else 1) * n/c pixels, eps_ld] (uncond half first), c channels

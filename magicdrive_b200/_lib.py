@@ -32,6 +32,7 @@ class GemmDesc(C.Structure):
         ("ln_stats", C.c_void_p), ("ln_parts", C.c_int), ("ln_eps", C.c_float), ("ln_colsum", C.c_void_p),
         ("stats_out", C.c_void_p),
         ("pad_h_end", C.c_int), ("pad_w_end", C.c_int),
+        ("operand_dtype", C.c_int),
     ]
 
 
@@ -48,23 +49,30 @@ SIGNATURES = {
     "mdb_gemm_conv_plan": (_i, [C.POINTER(GemmDesc), C.POINTER(C.c_int)]),
     "mdb_conv_direct": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp]),
     "mdb_groupnorm": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp, _i, _vp, _i, _vp, _vp]),
+    "mdb_groupnorm_f16": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp, _i, _vp, _i, _vp, _vp]),
     "mdb_layernorm": (_i, [_vp, _ll, _i, _i, _vp, _vp, _f, _vp, _i, _vp]),
     "mdb_attention": (_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _f, _vp]),
     "mdb_attention_multi": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _f, _vp]),
     "mdb_attention_varlen": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _f, _vp]),
+    "mdb_attention_varlen_f16": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _f, _vp]),
     "mdb_attention_causal":(_i, [_vp, _i, _vp, _i, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _f, _vp]),
     "mdb_clip_embed": (_i, [_vp, _i, _i, _i, _vp, _i, _vp, _i, _vp, _i, _vp, _vp]),
     "mdb_add": (_i, [_vp, _vp, _vp, _ll, _vp]),
+    "mdb_add_f16": (_i, [_vp, _vp, _vp, _ll, _vp]),
     "mdb_upsample_nearest": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp]),
     "mdb_adaptive_avgpool": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),
     "mdb_linear_small": (_i, [_vp, _i, _i, _i, _vp, _i, _vp, _i, _i, _i, _vp, _i, _vp]),
+    "mdb_linear_small_f16": (_i, [_vp, _i, _i, _i, _vp, _i, _vp, _i, _i, _i, _vp, _i, _vp]),
     "mdb_timestep_embedding": (_i, [_vp, _i, _i, _i, _f, _vp, _vp]),
     "mdb_fourier_embed": (_i, [_vp, _ll, _i, _i, _vp, _vp]),
     "mdb_nchw_to_nhwc": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
     "mdb_nhwc_to_nchw": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _vp]),
     "mdb_f32_to_bf16": (_i, [_vp, _vp, _ll, _vp]),
     "mdb_bf16_to_f32": (_i, [_vp, _vp, _ll, _vp]),
+    "mdb_f32_to_f16": (_i, [_vp, _vp, _ll, _vp]),
+    "mdb_f16_to_f32": (_i, [_vp, _vp, _ll, _vp]),
     "mdb_pack_latents": (_i, [_vp, _i, _ll, _i, _i, _i, _vp, _vp]),
+    "mdb_pack_latents_f16": (_i, [_vp, _i, _ll, _i, _i, _i, _vp, _vp]),
     "mdb_cfg_ddim_step": (_i, [_vp, _i, _i, _i, _f, _vp, _vp, _ll, _vp]),
     "mdb_softmax_rows": (_i, [_vp, _i, _ll, _i, _vp, _i, _i, _vp]),
     "mdb_pin_views": (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp, _ll, _i, _vp]),

@@ -38,7 +38,7 @@ struct AttnKvMaps {
 };
 
 struct AttnParams {
-  __nv_bfloat16* out;
+  void* out;  // bf16, or f16 in the F16 instantiations
   int ldo;
   int lq, lk;
   const int* kv_index;  // [b, n_sets]: (source << 24) | batch, or < 0 for an empty slot; nullptr = batch b, one set
@@ -70,10 +70,13 @@ struct AttnCfg {
   static_assert(STAGES >= 1 && kSmemBytes <= 232448, "shared memory");
 };
 
-template <int D, int BN_, bool CAUSAL = false, bool KVRES = false>
+// F16: f16 Q/K/V and output (fp16 models); P is packed to f16 pairs for the P V product, the softmax stays fp32.
+template <int D, int BN_, bool CAUSAL = false, bool KVRES = false, bool F16 = false>
 __global__ void __launch_bounds__(AttnCfg<D, BN_>::kThreads, 1)
 attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ AttnKvMaps kvm, const AttnParams p) {
   using Cfg = AttnCfg<D, BN_>;
+  using A = Act<F16>;
+  using Elt = typename A::T;
   constexpr int KD = Cfg::KD, D16 = Cfg::D16, BN = Cfg::BN, STAGES = Cfg::STAGES;
   constexpr int TILE_Q = Cfg::TILE_Q, TILE_KV = Cfg::TILE_KV;
   extern __shared__ uint8_t smem_raw[];
@@ -189,7 +192,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
           const int c = k / 4, kk = k % 4;
           const uint64_t adesc = make_sw128_kmajor_desc(smem_u32(smQ + c * TILE_Q + wg * (64 * 128))) + 2 * kk;
           const uint64_t bdesc = make_sw128_kmajor_desc(smem_u32(smK + (st * KD + c) * TILE_KV)) + 2 * kk;
-          WgmmaSS<BN>::run(s, adesc, bdesc, k > 0 ? 1u : 0u);
+          WgmmaSS<BN, F16>::run(s, adesc, bdesc, k > 0 ? 1u : 0u);
         }
         wgmma_commit();
         wgmma_wait<0>();
@@ -239,7 +242,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
             const float p0 = exp2f(fmaf(s[i0], sc, -m[h]));
             const float p1 = exp2f(fmaf(s[i0 + 1], sc, -m[h]));
             rs[h] += p0 + p1;
-            pa[kk][r] = pack_bf16(p0, p1);
+            pa[kk][r] = A::pack(p0, p1);
           }
         }
 #pragma unroll
@@ -254,7 +257,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
 #pragma unroll
         for (int kk = 0; kk < BN / 16; ++kk) {
           const uint64_t bdesc = make_sw128_mnmajor_desc(smem_u32(smV + st * KD * TILE_KV), TILE_KV) + (2048u >> 4) * kk;
-          WgmmaRSBmn<D16>::run(oacc, pa[kk], bdesc, 1u);
+          WgmmaRSBmn<D16, F16>::run(oacc, pa[kk], bdesc, 1u);
         }
         wgmma_commit();
         wgmma_wait<0>();
@@ -277,19 +280,19 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
       for (int h = 0; h < 2; ++h) {
         const int qrow = q0 + rloc + 8 * h;
         if (qrow >= p.lq) continue;
-        __nv_bfloat16* orow = p.out + (static_cast<long long>(b) * p.lq + qrow) * p.ldo + head * D;
+        Elt* orow = static_cast<Elt*>(p.out) + (static_cast<long long>(b) * p.lq + qrow) * p.ldo + head * D;
 #pragma unroll
         for (int g = 0; g < D16 / 8; ++g) {
           const int col = 8 * g + 2 * q;
           if (col >= D) continue;
           float f0 = oacc[4 * g + 2 * h] * inv[h], f1 = oacc[4 * g + 2 * h + 1] * inv[h];
           if (wrote) {
-            // every branch rounded to bf16 before the sum, like the reference's per-branch attention outputs
-            const float2 pf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(orow + col));
-            f0 = __bfloat162float(__float2bfloat16_rn(f0)) + pf.x;
-            f1 = __bfloat162float(__float2bfloat16_rn(f1)) + pf.y;
+            // every branch rounded to the storage type before the sum, like the reference's per-branch attention outputs
+            const float2 pf = A::to_float2(*reinterpret_cast<const typename A::T2*>(orow + col));
+            f0 = A::to_float(A::from_float(f0)) + pf.x;
+            f1 = A::to_float(A::from_float(f1)) + pf.y;
           }
-          *reinterpret_cast<uint32_t*>(orow + col) = pack_bf16(f0, f1);
+          *reinterpret_cast<uint32_t*>(orow + col) = A::pack(f0, f1);
         }
       }
       wrote = true;
@@ -299,7 +302,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
       for (int h = 0; h < 2; ++h) {
         const int qrow = q0 + rloc + 8 * h;
         if (qrow >= p.lq) continue;
-        __nv_bfloat16* orow = p.out + (static_cast<long long>(b) * p.lq + qrow) * p.ldo + head * D;
+        Elt* orow = static_cast<Elt*>(p.out) + (static_cast<long long>(b) * p.lq + qrow) * p.ldo + head * D;
 #pragma unroll
         for (int g = 0; g < D16 / 8; ++g)
           if (8 * g + 2 * q < D) *reinterpret_cast<uint32_t*>(orow + 8 * g + 2 * q) = 0u;

@@ -19,6 +19,11 @@ namespace {
 // A operand of a convolution: 4-D (C, W, H, N) im2col map, innermost first; pixel stride = ld elements.  The bounding box
 // of filter-tap-(0, 0) positions runs from -pad to (extent - 1 + pad + pad_end - (taps - 1)) in each spatial dimension,
 // walked with the stride: exactly h_out x w_out positions per image.
+// operand element type of a descriptor (mdb_gemm_desc.operand_dtype: 0 bf16, 1 f16)
+CUtensorMapDataType operand_type(const mdb_gemm_desc* d) {
+  return d->operand_dtype == 1 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+}
+
 bool make_im2col_map(CUtensorMap* m, const void* ptr, int c, int ld, const mdb_gemm_desc* d) {
   EncodeIm2colFn enc = get_encode_im2col();
   if (!enc) return false;
@@ -28,21 +33,21 @@ bool make_im2col_map(CUtensorMap* m, const void* ptr, int c, int ld, const mdb_g
   int lower[2] = {-d->pad_w, -d->pad_h};
   int upper[2] = {d->pad_w + d->pad_w_end - (d->taps_w - 1), d->pad_h + d->pad_h_end - (d->taps_h - 1)};
   cuuint32_t estr[4] = {1u, (cuuint32_t)d->stride, (cuuint32_t)d->stride, 1u};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, lower, upper, 64u,
+  CUresult r = enc(m, operand_type(d), 4, const_cast<void*>(ptr), dims, strides, lower, upper, 64u,
                    (cuuint32_t)kBlockM, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS;
 }
 
 // A operand of a 1x1 / stride-1 launch: 2-D [pixels, C] map, row stride ld elements.
-bool make_rows_map(CUtensorMap* m, const void* ptr, int c, int ld, long long pixels) {
+bool make_rows_map(CUtensorMap* m, const void* ptr, int c, int ld, long long pixels, CUtensorMapDataType dt) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return false;
   cuuint64_t dims[2] = {(cuuint64_t)c, (cuuint64_t)pixels};
   cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
   cuuint32_t box[2] = {64u, (cuuint32_t)kBlockM};
   cuuint32_t estr[2] = {1u, 1u};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+  CUresult r = enc(m, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS;
@@ -50,17 +55,17 @@ bool make_rows_map(CUtensorMap* m, const void* ptr, int c, int ld, long long pix
 
 bool make_act_map(CUtensorMap* m, const void* ptr, int c, int ld, const mdb_gemm_desc* d, bool im2col) {
   return im2col ? make_im2col_map(m, ptr, c, ld, d)
-                : make_rows_map(m, ptr, c, ld, (long long)d->n_img * d->h_out * d->w_out);
+                : make_rows_map(m, ptr, c, ld, (long long)d->n_img * d->h_out * d->w_out, operand_type(d));
 }
 
-bool make_w_map(CUtensorMap* m, const void* ptr, int n_out, int k, int block_n) {
+bool make_w_map(CUtensorMap* m, const void* ptr, int n_out, int k, int block_n, CUtensorMapDataType dt) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return false;
   cuuint64_t dims[2] = {(cuuint64_t)k, (cuuint64_t)n_out};
   cuuint64_t strides[1] = {(cuuint64_t)k * 2};
   cuuint32_t box[2] = {64u, (cuuint32_t)block_n};
   cuuint32_t estr[2] = {1u, 1u};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+  CUresult r = enc(m, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS;
@@ -114,6 +119,11 @@ int validate(const mdb_gemm_desc* d) {
                                           "(no residual, per-image shift or row statistics)");
   if (d->epi_mode < 0 || d->epi_mode > 3)
     return set_error(MDB_ERR_INVALID, "mdb_gemm_conv: epi_mode must be 0, 1, 2 or 3");
+  if (d->operand_dtype != 0 && d->operand_dtype != 1)
+    return set_error(MDB_ERR_INVALID, "mdb_gemm_conv: operand_dtype must be 0 (bf16) or 1 (f16)");
+  if (d->operand_dtype == 1 && (d->epi_mode == 2 || d->epi_mode == 3 || d->kernel_variant == 3))
+    return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: f16 operands take the linear and GEGLU epilogues on single CTAs "
+                                          "(no quick-GELU, ReLU or CTA pairs)");
   if (d->pad_h_end < 0 || d->pad_w_end < 0)
     return set_error(MDB_ERR_INVALID, "mdb_gemm_conv: end padding must not be negative (pad_h_end=%d pad_w_end=%d)",
                      d->pad_h_end, d->pad_w_end);
@@ -189,12 +199,12 @@ void make_plan(const mdb_gemm_desc* d, Plan* pl) {
   plan_for(d, 1, d->kernel_variant != 4, pl);
 }
 
-template <int BN, int CTAS, bool RELU>
+template <int BN, int CTAS, bool RELU, bool F16>
 int launch(const CUtensorMap& tA0, const CUtensorMap& tA1, const CUtensorMap& tB, const GemmParams& gp, cudaStream_t st) {
   using Cfg = WgGemmCfg<BN, CTAS>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, CTAS, RELU>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, CTAS, RELU, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Cfg::kSmemBytes);
     if (e != cudaSuccess) return set_error(MDB_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     attr_set = true;
@@ -213,21 +223,23 @@ int launch(const CUtensorMap& tA0, const CUtensorMap& tA1, const CUtensorMap& tB
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   add_pdl_attr(cfg, attr, 1);
-  cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<BN, CTAS, RELU>, tA0, tA1, tB, gp);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<BN, CTAS, RELU, F16>, tA0, tA1, tB, gp);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(MDB_ERR_CUDA, "gemm_wgmma_kernel<%d,%d> launch: %s", BN, CTAS, cudaGetErrorString(e));
   return MDB_OK;
 }
 
-template <int CTAS, bool RELU = false>
+template <int CTAS, bool RELU = false, bool F16 = false>
 int launch_bn(int block_n, const CUtensorMap& tA0, const CUtensorMap& tA1, const CUtensorMap& tB, const GemmParams& gp,
               cudaStream_t st) {
-  if (!RELU && gp.epi_mode == EPI_RELU) return launch_bn<CTAS, true>(block_n, tA0, tA1, tB, gp, st);
+  if constexpr (!F16) {  // f16 launches never take the ReLU epilogue (validate)
+    if (!RELU && gp.epi_mode == EPI_RELU) return launch_bn<CTAS, true>(block_n, tA0, tA1, tB, gp, st);
+  }
   switch (block_n) {
-    case 256: return launch<256, CTAS, RELU>(tA0, tA1, tB, gp, st);
-    case 160: return launch<160, CTAS, RELU>(tA0, tA1, tB, gp, st);
-    case 128: return launch<128, CTAS, RELU>(tA0, tA1, tB, gp, st);
-    case 64: return launch<64, CTAS, RELU>(tA0, tA1, tB, gp, st);
+    case 256: return launch<256, CTAS, RELU, F16>(tA0, tA1, tB, gp, st);
+    case 160: return launch<160, CTAS, RELU, F16>(tA0, tA1, tB, gp, st);
+    case 128: return launch<128, CTAS, RELU, F16>(tA0, tA1, tB, gp, st);
+    case 64: return launch<64, CTAS, RELU, F16>(tA0, tA1, tB, gp, st);
     default: return set_error(MDB_ERR_UNSUPPORTED, "mdb_gemm_conv: unsupported block_n %d", block_n);
   }
 }
@@ -287,7 +299,7 @@ extern "C" int mdb_gemm_conv(const mdb_gemm_desc* d, void* stream) {
     tA1 = tA0;
   }
   const int ktot = d->taps_h * d->taps_w * kBlockK * (cblocks(d->c0) + cblocks(d->c1));
-  if (!make_w_map(&tB, d->w, d->n_out, ktot, pl.block_n / pl.ctas))
+  if (!make_w_map(&tB, d->w, d->n_out, ktot, pl.block_n / pl.ctas, operand_type(d)))
     return set_error(MDB_ERR_CUDA, "cuTensorMapEncodeTiled(W) failed (n=%d k=%d)", d->n_out, ktot);
 
   GemmParams gp;
@@ -305,25 +317,33 @@ extern "C" int mdb_gemm_conv(const mdb_gemm_desc* d, void* stream) {
                                    : d->epi_mode;
   gp.out_is_f32 = d->out_is_f32;
   gp.bias = d->bias, gp.rowbias = d->rowbias, gp.rowbias_ld = d->rowbias_ld;
-  gp.residual = static_cast<const __nv_bfloat16*>(d->residual), gp.ldr = d->ldr;
+  gp.residual = d->residual, gp.ldr = d->ldr;
   gp.out = d->out, gp.ldo = d->ldo, gp.out_scale = d->out_scale;
   gp.partial = static_cast<float*>(d->workspace);
   gp.ln_stats = d->ln_stats, gp.ln_parts = d->ln_parts, gp.ln_eps = d->ln_eps, gp.ln_colsum = d->ln_colsum;
   gp.ln_inv_c = 1.0f / (float)(d->c0 + d->c1);
   gp.stats_out = d->stats_out;
 
-  rc = pl.ctas == 2 ? launch_bn<2>(pl.block_n, tA0, tA1, tB, gp, st) : launch_bn<1>(pl.block_n, tA0, tA1, tB, gp, st);
+  const bool f16 = d->operand_dtype == 1;
+  rc = pl.ctas == 2 ? launch_bn<2>(pl.block_n, tA0, tA1, tB, gp, st)
+       : f16        ? launch_bn<1, false, true>(pl.block_n, tA0, tA1, tB, gp, st)
+                    : launch_bn<1>(pl.block_n, tA0, tA1, tB, gp, st);
   if (rc != MDB_OK) return rc;
   if (pl.splits > 1) {
     const long long pixels = (long long)d->n_img * d->h_out * d->w_out;
     const long long total4 = pixels * d->n_out / 4;
     const int threads = 256;
     const int blocks = (int)((total4 + threads - 1) / threads);
-    cudaError_t e = launch_pdl(d->epi_mode == 3 ? splitk_finalize_kernel<true> : splitk_finalize_kernel<false>, dim3(blocks),
-                               dim3(threads), 0, st, static_cast<const float*>(d->workspace), pl.splits, pixels, d->n_out,
-                               d->h_out * d->w_out, d->bias, d->rowbias, d->rowbias_ld,
-                               static_cast<const __nv_bfloat16*>(d->residual), d->ldr, d->out, d->ldo, d->out_is_f32,
-                               d->out_scale);
+    cudaError_t e =
+        f16 ? launch_pdl(splitk_finalize_kernel<false, true>, dim3(blocks), dim3(threads), 0, st,
+                         static_cast<const float*>(d->workspace), pl.splits, pixels, d->n_out, d->h_out * d->w_out, d->bias,
+                         d->rowbias, d->rowbias_ld, static_cast<const __half*>(d->residual), d->ldr, d->out, d->ldo,
+                         d->out_is_f32, d->out_scale)
+            : launch_pdl(d->epi_mode == 3 ? splitk_finalize_kernel<true> : splitk_finalize_kernel<false>, dim3(blocks),
+                         dim3(threads), 0, st, static_cast<const float*>(d->workspace), pl.splits, pixels, d->n_out,
+                         d->h_out * d->w_out, d->bias, d->rowbias, d->rowbias_ld,
+                         static_cast<const __nv_bfloat16*>(d->residual), d->ldr, d->out, d->ldo, d->out_is_f32,
+                         d->out_scale);
     if (e == cudaSuccess) e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(MDB_ERR_CUDA, "splitk_finalize launch: %s", cudaGetErrorString(e));
   }

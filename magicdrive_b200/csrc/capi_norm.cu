@@ -20,36 +20,41 @@
 
 namespace {
 
+// F16 (the GroupNorm kernels' template flag): f16 activations (fp16 models) in place of bf16; statistics stay fp32
+template <bool F16 = false>
 __device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
-  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
+  using A = mdb::Act<F16>;
+  const typename A::T2* h = reinterpret_cast<const typename A::T2*>(&u);
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
-    const float2 t = __bfloat1622float2(h[i]);
+    const float2 t = A::to_float2(h[i]);
     f[2 * i] = t.x, f[2 * i + 1] = t.y;
   }
 }
+template <bool F16 = false>
 __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
+  using A = mdb::Act<F16>;
   uint4 u;
-  __nv_bfloat162 h0 = __floats2bfloat162_rn(f[0], f[1]), h1 = __floats2bfloat162_rn(f[2], f[3]);
-  __nv_bfloat162 h2 = __floats2bfloat162_rn(f[4], f[5]), h3 = __floats2bfloat162_rn(f[6], f[7]);
-  u.x = *reinterpret_cast<uint32_t*>(&h0), u.y = *reinterpret_cast<uint32_t*>(&h1);
-  u.z = *reinterpret_cast<uint32_t*>(&h2), u.w = *reinterpret_cast<uint32_t*>(&h3);
+  u.x = A::pack(f[0], f[1]), u.y = A::pack(f[2], f[3]);
+  u.z = A::pack(f[4], f[5]), u.w = A::pack(f[6], f[7]);
   return u;
 }
 
 // Shift of group g of an image for the two-kernel statistics: the image's first pixel, first channel of the group.  Sums of
 // (x - shift) keep E[d^2] - E[d]^2 well conditioned: a sample of the group lies within a few standard deviations of its mean,
 // whereas the plain E[x^2] - mean^2 in fp32 is off by several percent once |mean| is a few hundred standard deviations.
-__device__ __forceinline__ float gn_shift(const __nv_bfloat16* __restrict__ x0, int c0, int ld0,
-                                          const __nv_bfloat16* __restrict__ x1, int ld1, long long pix, int c) {
-  return __bfloat162float(c < c0 ? x0[pix * ld0 + c] : x1[pix * ld1 + (c - c0)]);
+template <bool F16>
+__device__ __forceinline__ float gn_shift(const typename mdb::Act<F16>::T* __restrict__ x0, int c0, int ld0,
+                                          const typename mdb::Act<F16>::T* __restrict__ x1, int ld1, long long pix, int c) {
+  return mdb::Act<F16>::to_float(c < c0 ? x0[pix * ld0 + c] : x1[pix * ld1 + (c - c0)]);
 }
 
 // ---- GroupNorm pass 1: per (image, group) sum / sum-of-squares of x - shift.  blockDim = vpp * R, thread = (pixel lane r,
 // channel vector cv)
-__global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x0, int c0, int ld0,
-                                const __nv_bfloat16* __restrict__ x1, int c1, int ld1, int hw, int groups, int vpp,
-                                int R, int pix_per_cta, float* __restrict__ stats) {
+template <bool F16>
+__device__ __forceinline__ void gn_stats(const typename mdb::Act<F16>::T* __restrict__ x0, int c0, int ld0,
+                                         const typename mdb::Act<F16>::T* __restrict__ x1, int c1, int ld1, int hw, int groups,
+                                         int vpp, int R, int pix_per_cta, float* __restrict__ stats) {
   extern __shared__ float sm[];  // [2][ctot]
   const int ctot = c0 + c1;
   const int cpg = ctot / groups;
@@ -62,7 +67,7 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x0, int c0, in
   const int r = threadIdx.x / vpp;
   if (r < R) {
     const int ch = cv * 8;
-    const __nv_bfloat16* base;
+    const typename mdb::Act<F16>::T* base;
     int ld, coff;
     if (ch < c0) base = x0, ld = ld0, coff = ch;
     else base = x1, ld = ld1, coff = ch - c0;
@@ -70,12 +75,12 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x0, int c0, in
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       s[i] = 0.f, ss[i] = 0.f;
-      k[i] = gn_shift(x0, c0, ld0, x1, ld1, static_cast<long long>(img) * hw, (ch + i) / cpg * cpg);
+      k[i] = gn_shift<F16>(x0, c0, ld0, x1, ld1, static_cast<long long>(img) * hw, (ch + i) / cpg * cpg);
     }
     for (int p = p_begin + r; p < p_end; p += R) {
       const uint4 u = __ldg(reinterpret_cast<const uint4*>(base + (static_cast<long long>(img) * hw + p) * ld + coff));
       float f[8];
-      unpack8(u, f);
+      unpack8<F16>(u, f);
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         const float d = f[i] - k[i];
@@ -97,13 +102,23 @@ __global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x0, int c0, in
   }
 }
 
+__global__ void gn_stats_kernel(const __nv_bfloat16* __restrict__ x0, int c0, int ld0, const __nv_bfloat16* __restrict__ x1,
+                                int c1, int ld1, int hw, int groups, int vpp, int R, int pix_per_cta, float* __restrict__ stats) {
+  gn_stats<false>(x0, c0, ld0, x1, c1, ld1, hw, groups, vpp, R, pix_per_cta, stats);
+}
+__global__ void gn_stats_f16_kernel(const __half* __restrict__ x0, int c0, int ld0, const __half* __restrict__ x1, int c1,
+                                    int ld1, int hw, int groups, int vpp, int R, int pix_per_cta, float* __restrict__ stats) {
+  gn_stats<true>(x0, c0, ld0, x1, c1, ld1, hw, groups, vpp, R, pix_per_cta, stats);
+}
+
 // ---- GroupNorm pass 2: mean = shift + E[x - shift], var = E[(x - shift)^2] - E[x - shift]^2;
 // y = (x - mean) * rstd * gamma + beta, optional SiLU, bf16 out.
-__global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x0, int c0, int ld0,
-                                const __nv_bfloat16* __restrict__ x1, int c1, int ld1, int hw, int groups, float eps,
-                                const float* __restrict__ gamma, const float* __restrict__ beta, int silu,
-                                const float* __restrict__ stats, __nv_bfloat16* __restrict__ out, int ldo,
-                                int pix_per_cta) {
+template <bool F16>
+__device__ __forceinline__ void gn_apply(const typename mdb::Act<F16>::T* __restrict__ x0, int c0, int ld0,
+                                         const typename mdb::Act<F16>::T* __restrict__ x1, int c1, int ld1, int hw, int groups,
+                                         float eps, const float* __restrict__ gamma, const float* __restrict__ beta, int silu,
+                                         const float* __restrict__ stats, typename mdb::Act<F16>::T* __restrict__ out, int ldo,
+                                         int pix_per_cta) {
   extern __shared__ float sm[];  // scale[ctot], shift[ctot]
   const int ctot = c0 + c1;
   const int img = blockIdx.y;
@@ -114,7 +129,7 @@ __global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x0, int c0, in
     const float dmean = stats[(img * groups + g) * 2] * inv_cnt;  // mean of x - shift
     float var = stats[(img * groups + g) * 2 + 1] * inv_cnt - dmean * dmean;
     var = fmaxf(var, 0.f);
-    const float mean = gn_shift(x0, c0, ld0, x1, ld1, static_cast<long long>(img) * hw, g * cpg) + dmean;
+    const float mean = gn_shift<F16>(x0, c0, ld0, x1, ld1, static_cast<long long>(img) * hw, g * cpg) + dmean;
     const float rstd = rsqrtf(var + eps);
     const float a = rstd * gamma[c];
     sm[c] = a;
@@ -132,15 +147,28 @@ __global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x0, int c0, in
     const uint4 u = (ch < c0) ? __ldg(reinterpret_cast<const uint4*>(x0 + pix * ld0 + ch))
                               : __ldg(reinterpret_cast<const uint4*>(x1 + pix * ld1 + (ch - c0)));
     float f[8];
-    unpack8(u, f);
+    unpack8<F16>(u, f);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       float y = f[i] * sm[ch + i] + sm[ctot + ch + i];
       if (silu) y = y / (1.0f + __expf(-y));
       f[i] = y;
     }
-    *reinterpret_cast<uint4*>(out + pix * ldo + ch) = pack8(f);
+    *reinterpret_cast<uint4*>(out + pix * ldo + ch) = pack8<F16>(f);
   }
+}
+
+__global__ void gn_apply_kernel(const __nv_bfloat16* __restrict__ x0, int c0, int ld0, const __nv_bfloat16* __restrict__ x1,
+                                int c1, int ld1, int hw, int groups, float eps, const float* __restrict__ gamma,
+                                const float* __restrict__ beta, int silu, const float* __restrict__ stats,
+                                __nv_bfloat16* __restrict__ out, int ldo, int pix_per_cta) {
+  gn_apply<false>(x0, c0, ld0, x1, c1, ld1, hw, groups, eps, gamma, beta, silu, stats, out, ldo, pix_per_cta);
+}
+__global__ void gn_apply_f16_kernel(const __half* __restrict__ x0, int c0, int ld0, const __half* __restrict__ x1, int c1,
+                                    int ld1, int hw, int groups, float eps, const float* __restrict__ gamma,
+                                    const float* __restrict__ beta, int silu, const float* __restrict__ stats,
+                                    __half* __restrict__ out, int ldo, int pix_per_cta) {
+  gn_apply<true>(x0, c0, ld0, x1, c1, ld1, hw, groups, eps, gamma, beta, silu, stats, out, ldo, pix_per_cta);
 }
 
 // ---- GroupNorm, single kernel: one CTA per (image, group).  The group's hw x cpg slab (a few tens of KB, L2-resident:
@@ -154,16 +182,18 @@ __device__ __forceinline__ void cp_async4(void* dst_smem, const void* src) {
                : "memory");
 }
 
-template <bool CACHED>
-__global__ void __launch_bounds__(256) gn_fused_kernel(const __nv_bfloat16* __restrict__ x0, int c0, int ld0,
-                                                       const __nv_bfloat16* __restrict__ x1, int c1, int ld1, int hw,
+template <bool CACHED, bool F16 = false>
+__global__ void __launch_bounds__(256) gn_fused_kernel(const typename mdb::Act<F16>::T* __restrict__ x0, int c0, int ld0,
+                                                       const typename mdb::Act<F16>::T* __restrict__ x1, int c1, int ld1, int hw,
                                                        int groups, float eps, const float* __restrict__ gamma,
                                                        const float* __restrict__ beta, int silu,
-                                                       __nv_bfloat16* __restrict__ out, int ldo, uint32_t inv_pp) {
+                                                       typename mdb::Act<F16>::T* __restrict__ out, int ldo, uint32_t inv_pp) {
+  using A = mdb::Act<F16>;
   constexpr int T = 256;
   mdb::pdl_wait();
   mdb::pdl_launch_dependents();
-  extern __shared__ uint32_t slab[];  // [units] bf16x2 (CACHED only)
+  // [units] bf16x2 / f16x2 (CACHED only); 128-byte aligned like gn_rows_kernel's slab, which shares the dynamic region
+  extern __shared__ __align__(128) uint32_t slab[];
   __shared__ float red[T / 32];
   __shared__ float bcast;
   const int g = blockIdx.x, img = blockIdx.y;
@@ -186,7 +216,7 @@ __global__ void __launch_bounds__(256) gn_fused_kernel(const __nv_bfloat16* __re
   };
   auto value = [&](int u) -> float2 {
     const uint32_t w = CACHED ? slab[u] : __ldg(src(u));
-    return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w));
+    return A::to_float2(*reinterpret_cast<const typename A::T2*>(&w));
   };
   auto block_sum = [&](float v) -> float {
 #pragma unroll
@@ -238,8 +268,7 @@ __global__ void __launch_bounds__(256) gn_fused_kernel(const __nv_bfloat16* __re
       y0 = y0 / (1.0f + __expf(-y0));
       y1 = y1 / (1.0f + __expf(-y1));
     }
-    __nv_bfloat162 h = __floats2bfloat162_rn(y0, y1);
-    *reinterpret_cast<uint32_t*>(out + (pix0 + p) * ldo + c) = *reinterpret_cast<uint32_t*>(&h);
+    *reinterpret_cast<uint32_t*>(out + (pix0 + p) * ldo + c) = A::pack(y0, y1);
   }
 }
 
@@ -318,11 +347,14 @@ __device__ __forceinline__ float ld_dsmem_f32(uint32_t cluster_addr) {
   asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(cluster_addr));
   return v;
 }
-__global__ void gn_rows_kernel(const __nv_bfloat16* __restrict__ x0, int c0, int ld0, const __nv_bfloat16* __restrict__ x1,
-                               int c1, int ld1, int hw, int groups, float eps, const float* __restrict__ gamma,
-                               const float* __restrict__ beta, int silu, __nv_bfloat16* __restrict__ out, int ldo, int vpp, int R,
-                               int ctas_per_img, int pix_per_cta) {
+template <bool F16>
+__device__ __forceinline__ void gn_rows(const typename mdb::Act<F16>::T* __restrict__ x0, int c0, int ld0,
+                                        const typename mdb::Act<F16>::T* __restrict__ x1, int c1, int ld1, int hw, int groups,
+                                        float eps, const float* __restrict__ gamma, const float* __restrict__ beta, int silu,
+                                        typename mdb::Act<F16>::T* __restrict__ out, int ldo, int vpp, int R, int ctas_per_img,
+                                        int pix_per_cta) {
   using namespace mdb;
+  using Elt = typename Act<F16>::T;
   extern __shared__ __align__(128) uint4 gslab[];  // [pix_per_cta][c0] | [pix_per_cta][c1] bf16, then float red[R][ctot]
   const int ctot = c0 + c1, cpg = ctot / groups;
   float* red = reinterpret_cast<float*>(gslab + static_cast<size_t>(pix_per_cta) * vpp);  // [R][ctot]
@@ -352,7 +384,7 @@ __global__ void gn_rows_kernel(const __nv_bfloat16* __restrict__ x0, int c0, int
   // All copies complete on full_bar.
   {
     const uint32_t bar = smem_u32(&full_bar);
-    auto fetch = [&](const __nv_bfloat16* src, int c, int ld, uint32_t dst) {
+    auto fetch = [&](const Elt* src, int c, int ld, uint32_t dst) {
       if (c == 0) return;
       if (ld == c) {
         const uint32_t bytes = static_cast<uint32_t>(npix) * c * 2;
@@ -379,7 +411,7 @@ __global__ void gn_rows_kernel(const __nv_bfloat16* __restrict__ x0, int c0, int
   float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   for (int p = r0; p < npix; p += R) {
     float f[8];
-    unpack8(mine[p * pitch], f);
+    unpack8<F16>(mine[p * pitch], f);
 #pragma unroll
     for (int e = 0; e < 8; ++e) acc[e] += f[e];
   }
@@ -405,7 +437,7 @@ __global__ void gn_rows_kernel(const __nv_bfloat16* __restrict__ x0, int c0, int
   for (int e = 0; e < 8; ++e) lm[e] = part[2 * ((ch + e) / cpg)], acc[e] = 0.f;
   for (int p = r0; p < npix; p += R) {
     float f[8];
-    unpack8(mine[p * pitch], f);
+    unpack8<F16>(mine[p * pitch], f);
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
       const float d = f[e] - lm[e];
@@ -464,27 +496,55 @@ __global__ void gn_rows_kernel(const __nv_bfloat16* __restrict__ x0, int c0, int
     sa[e] = rs * __ldg(gamma + ch + e);
     sb[e] = __ldg(beta + ch + e) - mu * sa[e];
   }
-  __nv_bfloat16* dst = out + pix0 * ldo + ch;
+  Elt* dst = out + pix0 * ldo + ch;
   for (int p = r0; p < npix; p += R) {
     float f[8];
-    unpack8(mine[p * pitch], f);
+    unpack8<F16>(mine[p * pitch], f);
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
       float y = fmaf(f[e], sa[e], sb[e]);
       if (silu) y = y / (1.0f + __expf(-y));
       f[e] = y;
     }
-    *reinterpret_cast<uint4*>(dst + static_cast<long long>(p) * ldo) = pack8(f);
+    *reinterpret_cast<uint4*>(dst + static_cast<long long>(p) * ldo) = pack8<F16>(f);
   }
   if (ctas_per_img > 1) asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-}  // namespace
+__global__ void gn_rows_kernel(const __nv_bfloat16* __restrict__ x0, int c0, int ld0, const __nv_bfloat16* __restrict__ x1,
+                               int c1, int ld1, int hw, int groups, float eps, const float* __restrict__ gamma,
+                               const float* __restrict__ beta, int silu, __nv_bfloat16* __restrict__ out, int ldo, int vpp, int R,
+                               int ctas_per_img, int pix_per_cta) {
+  gn_rows<false>(x0, c0, ld0, x1, c1, ld1, hw, groups, eps, gamma, beta, silu, out, ldo, vpp, R, ctas_per_img, pix_per_cta);
+}
+__global__ void gn_rows_f16_kernel(const __half* __restrict__ x0, int c0, int ld0, const __half* __restrict__ x1, int c1,
+                                   int ld1, int hw, int groups, float eps, const float* __restrict__ gamma,
+                                   const float* __restrict__ beta, int silu, __half* __restrict__ out, int ldo, int vpp, int R,
+                                   int ctas_per_img, int pix_per_cta) {
+  gn_rows<true>(x0, c0, ld0, x1, c1, ld1, hw, groups, eps, gamma, beta, silu, out, ldo, vpp, R, ctas_per_img, pix_per_cta);
+}
 
-extern "C" int mdb_groupnorm(const void* x0, int c0, int ld0, const void* x1, int c1, int ld1, int n_img, int hw,
-                             int groups, float eps, const float* gamma, const float* beta, int silu, void* out, int ldo,
-                             float* stats_ws, void* stream) {
+// the plain kernels of one element type (plain, not templates: the bf16 ones compile as they did before f16 existed)
+template <bool F16> struct GnKernels {
+  static constexpr auto stats = gn_stats_kernel;
+  static constexpr auto apply = gn_apply_kernel;
+  static constexpr auto rows = gn_rows_kernel;
+};
+template <> struct GnKernels<true> {
+  static constexpr auto stats = gn_stats_f16_kernel;
+  static constexpr auto apply = gn_apply_f16_kernel;
+  static constexpr auto rows = gn_rows_f16_kernel;
+};
+
+// mdb_groupnorm (bf16) and mdb_groupnorm_f16: the same kernel choice for both element types
+template <bool F16>
+int groupnorm(const void* x0_, int c0, int ld0, const void* x1_, int c1, int ld1, int n_img, int hw, int groups, float eps,
+              const float* gamma, const float* beta, int silu, void* out_, int ldo, float* stats_ws, void* stream) {
   using namespace mdb;
+  using Elt = typename Act<F16>::T;
+  const Elt* x0 = static_cast<const Elt*>(x0_);
+  const Elt* x1 = static_cast<const Elt*>(x1_);
+  Elt* out = static_cast<Elt*>(out_);
   const int ctot = c0 + c1;
   if (!x0 || !out || !stats_ws || !gamma || !beta) return set_error(MDB_ERR_INVALID, "mdb_groupnorm: null pointer");
   if (c0 % 8 || c1 % 8 || ld0 % 8 || (c1 && ld1 % 8) || ldo % 8 || ctot % groups || ctot > 4096)
@@ -510,8 +570,8 @@ extern "C" int mdb_groupnorm(const void* x0, int c0, int ld0, const void* x1, in
       static bool attr = false;
       static int max16 = -1;  // >0: 16-CTA clusters of this kernel can be co-scheduled
       if (!attr) {
-        cudaFuncSetAttribute(gn_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kMaxSmem));
-        max16 = (cudaFuncSetAttribute(gn_rows_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess) ? 1 : 0;
+        cudaFuncSetAttribute(GnKernels<F16>::rows, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kMaxSmem));
+        max16 = (cudaFuncSetAttribute(GnKernels<F16>::rows, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) == cudaSuccess) ? 1 : 0;
         cudaGetLastError();
         attr = true;
       }
@@ -531,7 +591,7 @@ extern "C" int mdb_groupnorm(const void* x0, int c0, int ld0, const void* x1, in
           pa[0].val.clusterDim.x = cand, pa[0].val.clusterDim.y = 1, pa[0].val.clusterDim.z = 1;
           probe.attrs = pa, probe.numAttrs = 1;
           int n_clusters = 0;
-          const bool ok = cudaOccupancyMaxActiveClusters(&n_clusters, gn_rows_kernel, &probe) == cudaSuccess && n_clusters >= 1;
+          const bool ok = cudaOccupancyMaxActiveClusters(&n_clusters, GnKernels<F16>::rows, &probe) == cudaSuccess && n_clusters >= 1;
           cudaGetLastError();
           if (!ok) return false;
         }
@@ -550,9 +610,8 @@ extern "C" int mdb_groupnorm(const void* x0, int c0, int ld0, const void* x1, in
         la[0].id = cudaLaunchAttributeClusterDimension;
         la[0].val.clusterDim.x = cpi, la[0].val.clusterDim.y = 1, la[0].val.clusterDim.z = 1;
         add_pdl_attr(cfg, la, 1);
-        cudaError_t le = cudaLaunchKernelEx(&cfg, gn_rows_kernel, static_cast<const __nv_bfloat16*>(x0), c0, ld0,
-                                            static_cast<const __nv_bfloat16*>(x1), c1, ld1, hw, groups, eps, gamma, beta, silu,
-                                            static_cast<__nv_bfloat16*>(out), ldo, vpp, R, cpi, ppc);
+        cudaError_t le = cudaLaunchKernelEx(&cfg, GnKernels<F16>::rows, x0, c0, ld0, x1, c1, ld1, hw, groups, eps, gamma, beta,
+                                            silu, out, ldo, vpp, R, cpi, ppc);
         if (le != cudaSuccess) return set_error(MDB_ERR_CUDA, "gn_rows_kernel launch: %s", cudaGetErrorString(le));
         MDB_CHECK_LAUNCH("gn_rows_kernel");
         return MDB_OK;
@@ -568,16 +627,14 @@ extern "C" int mdb_groupnorm(const void* x0, int c0, int ld0, const void* x1, in
     if (slab_bytes <= 96 * 1024) {
       static bool attr = false;
       if (!attr) {
-        cudaFuncSetAttribute(gn_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
+        cudaFuncSetAttribute(gn_fused_kernel<true, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
         attr = true;
       }
-      launch_pdl(gn_fused_kernel<true>, dim3(groups, n_img), dim3(256), slab_bytes, st,
-                 static_cast<const __nv_bfloat16*>(x0), c0, ld0, static_cast<const __nv_bfloat16*>(x1), c1, ld1, hw, groups,
-                 eps, gamma, beta, silu, static_cast<__nv_bfloat16*>(out), ldo, inv_pp);
+      launch_pdl(gn_fused_kernel<true, F16>, dim3(groups, n_img), dim3(256), slab_bytes, st, x0, c0, ld0, x1, c1, ld1, hw,
+                 groups, eps, gamma, beta, silu, out, ldo, inv_pp);
     } else {
-      gn_fused_kernel<false><<<dim3(groups, n_img), 256, 0, st>>>(
-          static_cast<const __nv_bfloat16*>(x0), c0, ld0, static_cast<const __nv_bfloat16*>(x1), c1, ld1, hw, groups, eps,
-          gamma, beta, silu, static_cast<__nv_bfloat16*>(out), ldo, inv_pp);
+      gn_fused_kernel<false, F16><<<dim3(groups, n_img), 256, 0, st>>>(x0, c0, ld0, x1, c1, ld1, hw, groups, eps, gamma, beta,
+                                                                       silu, out, ldo, inv_pp);
     }
     MDB_CHECK_LAUNCH("gn_fused_kernel");
     return MDB_OK;
@@ -601,15 +658,27 @@ extern "C" int mdb_groupnorm(const void* x0, int c0, int ld0, const void* x1, in
   if (pix_per_cta < R) pix_per_cta = R;
   chunks = (hw + pix_per_cta - 1) / pix_per_cta;
   const size_t smem = sizeof(float) * 2 * ctot;
-  gn_stats_kernel<<<dim3(chunks, n_img), threads, smem, st>>>(
-      static_cast<const __nv_bfloat16*>(x0), c0, ld0, static_cast<const __nv_bfloat16*>(x1), c1, ld1, hw, groups, vpp,
-      R, pix_per_cta, stats_ws);
+  GnKernels<F16>::stats<<<dim3(chunks, n_img), threads, smem, st>>>(x0, c0, ld0, x1, c1, ld1, hw, groups, vpp, R, pix_per_cta,
+                                                                   stats_ws);
   MDB_CHECK_LAUNCH("gn_stats_kernel");
-  gn_apply_kernel<<<dim3(chunks, n_img), 256, smem, st>>>(
-      static_cast<const __nv_bfloat16*>(x0), c0, ld0, static_cast<const __nv_bfloat16*>(x1), c1, ld1, hw, groups, eps,
-      gamma, beta, silu, stats_ws, static_cast<__nv_bfloat16*>(out), ldo, pix_per_cta);
+  GnKernels<F16>::apply<<<dim3(chunks, n_img), 256, smem, st>>>(x0, c0, ld0, x1, c1, ld1, hw, groups, eps, gamma, beta, silu,
+                                                                 stats_ws, out, ldo, pix_per_cta);
   MDB_CHECK_LAUNCH("gn_apply_kernel");
   return MDB_OK;
+}
+
+}  // namespace
+
+extern "C" int mdb_groupnorm(const void* x0, int c0, int ld0, const void* x1, int c1, int ld1, int n_img, int hw,
+                             int groups, float eps, const float* gamma, const float* beta, int silu, void* out, int ldo,
+                             float* stats_ws, void* stream) {
+  return groupnorm<false>(x0, c0, ld0, x1, c1, ld1, n_img, hw, groups, eps, gamma, beta, silu, out, ldo, stats_ws, stream);
+}
+
+extern "C" int mdb_groupnorm_f16(const void* x0, int c0, int ld0, const void* x1, int c1, int ld1, int n_img, int hw,
+                                 int groups, float eps, const float* gamma, const float* beta, int silu, void* out, int ldo,
+                                 float* stats_ws, void* stream) {
+  return groupnorm<true>(x0, c0, ld0, x1, c1, ld1, n_img, hw, groups, eps, gamma, beta, silu, out, ldo, stats_ws, stream);
 }
 
 extern "C" int mdb_layernorm(const void* x, long long rows, int c, int ldx, const float* gamma, const float* beta,

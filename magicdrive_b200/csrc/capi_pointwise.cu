@@ -2,28 +2,39 @@
 // sinusoidal + Fourier embeddings, the skinny linear layers, the tiny-channel direct convolution and the fused
 // classifier-free-guidance + DDIM update.  Compiled WITHOUT --use_fast_math (sin/cos/exp/erf are exact-path).
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <math.h>
 
 #include "../../include/magicdrive_b200.h"
 #include "common_host.h"
+#include "ptx.cuh"
 
 namespace {
 
-__global__ void add_kernel(const uint4* __restrict__ a, const uint4* __restrict__ b, uint4* __restrict__ o, long long n8) {
+// F16: f16 elements (fp16 models) in place of bf16; the sum is taken in fp32 and rounded once
+template <bool F16>
+__device__ __forceinline__ void add8(const uint4* __restrict__ a, const uint4* __restrict__ b, uint4* __restrict__ o,
+                                     long long n8) {
+  using A = mdb::Act<F16>;
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= n8) return;
   const uint4 ua = __ldg(a + i), ub = __ldg(b + i);
-  const __nv_bfloat162* ha = reinterpret_cast<const __nv_bfloat162*>(&ua);
-  const __nv_bfloat162* hb = reinterpret_cast<const __nv_bfloat162*>(&ub);
-  uint4 r;
-  __nv_bfloat162* hr = reinterpret_cast<__nv_bfloat162*>(&r);
+  const typename A::T2* ha = reinterpret_cast<const typename A::T2*>(&ua);
+  const typename A::T2* hb = reinterpret_cast<const typename A::T2*>(&ub);
+  uint32_t r[4];
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
-    const float2 fa = __bfloat1622float2(ha[j]), fb = __bfloat1622float2(hb[j]);
-    hr[j] = __floats2bfloat162_rn(fa.x + fb.x, fa.y + fb.y);
+    const float2 fa = A::to_float2(ha[j]), fb = A::to_float2(hb[j]);
+    r[j] = A::pack(fa.x + fb.x, fa.y + fb.y);
   }
-  o[i] = r;
+  o[i] = make_uint4(r[0], r[1], r[2], r[3]);
+}
+__global__ void add_kernel(const uint4* __restrict__ a, const uint4* __restrict__ b, uint4* __restrict__ o, long long n8) {
+  add8<false>(a, b, o, n8);
+}
+__global__ void add_f16_kernel(const uint4* __restrict__ a, const uint4* __restrict__ b, uint4* __restrict__ o, long long n8) {
+  add8<true>(a, b, o, n8);
 }
 
 __global__ void upsample_nearest_kernel(const uint4* __restrict__ x, int n, int h, int w, int c8, uint4* __restrict__ o,
@@ -71,6 +82,8 @@ template <>
 __device__ __forceinline__ float ldf<float>(const float* p) { return *p; }
 template <>
 __device__ __forceinline__ float ldf<__nv_bfloat16>(const __nv_bfloat16* p) { return __bfloat162float(*p); }
+template <>
+__device__ __forceinline__ float ldf<__half>(const __half* p) { return __half2float(*p); }
 
 // NCHW -> NHWC through a 32x32 smem transpose tile over (c, hw)
 template <typename T>
@@ -114,6 +127,14 @@ __global__ void f32_to_bf16_kernel(const float* __restrict__ x, __nv_bfloat16* _
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i < n) o[i] = __float2bfloat16_rn(x[i]);
 }
+__global__ void f32_to_f16_kernel(const float* __restrict__ x, __half* __restrict__ o, long long n) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i < n) o[i] = __float2half_rn(x[i]);
+}
+__global__ void f16_to_f32_kernel(const __half* __restrict__ x, float* __restrict__ o, long long n) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i < n) o[i] = __half2float(x[i]);
+}
 __global__ void bf16_to_f32_kernel(const __nv_bfloat16* __restrict__ x, float* __restrict__ o, long long n) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i < n) o[i] = __bfloat162float(x[i]);
@@ -154,12 +175,15 @@ __global__ void fourier_kernel(const float* __restrict__ x, long long rows, int 
 
 __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + expf(-x)); }
 
-// Skinny linear: CTA = 8 warps x 4 columns; activations staged once per CTA in shared memory (fp32), weights bf16
-// streamed with 16-byte loads; rows processed in chunks of 16.
+// Skinny linear: CTA = 8 warps x 4 columns; activations staged once per CTA in shared memory (fp32), weights bf16 (f16 with
+// F16: the encoders of fp16 models) streamed with 16-byte loads; rows processed in chunks of 16.
 constexpr int LS_ROWS = 16;
-__global__ void linear_small_kernel(const float* __restrict__ in, int m, int k, int ldi, const __nv_bfloat16* __restrict__ w,
-                                    int ldw, const float* __restrict__ bias, int n, int pre_silu, int post_silu,
-                                    float* __restrict__ out, int ldo) {
+template <bool F16>
+__device__ __forceinline__ void linear_small(const float* __restrict__ in, int m, int k, int ldi,
+                                             const typename mdb::Act<F16>::T* __restrict__ w, int ldw,
+                                             const float* __restrict__ bias, int n, int pre_silu, int post_silu,
+                                             float* __restrict__ out, int ldo) {
+  using A = mdb::Act<F16>;
   extern __shared__ float s_in[];  // [LS_ROWS][k]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int col_base = blockIdx.x * 32 + warp * 4;
@@ -178,20 +202,20 @@ __global__ void linear_small_kernel(const float* __restrict__ in, int m, int k, 
       float acc[LS_ROWS];
 #pragma unroll
       for (int r = 0; r < LS_ROWS; ++r) acc[r] = 0.f;
-      const __nv_bfloat16* wr = w + static_cast<long long>(col) * ldw;
+      const typename A::T* wr = w + static_cast<long long>(col) * ldw;
       for (int kk = lane * 8; kk < k; kk += 256) {
         float wf[8];
         if (kk + 8 <= k && (ldw % 8) == 0) {
           const uint4 u = __ldg(reinterpret_cast<const uint4*>(wr + kk));
-          const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
+          const typename A::T2* h = reinterpret_cast<const typename A::T2*>(&u);
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
-            const float2 t = __bfloat1622float2(h[j]);
+            const float2 t = A::to_float2(h[j]);
             wf[2 * j] = t.x, wf[2 * j + 1] = t.y;
           }
         } else {
 #pragma unroll
-          for (int j = 0; j < 8; ++j) wf[j] = (kk + j < k) ? __bfloat162float(wr[kk + j]) : 0.f;
+          for (int j = 0; j < 8; ++j) wf[j] = (kk + j < k) ? A::to_float(wr[kk + j]) : 0.f;
         }
 #pragma unroll
         for (int r = 0; r < LS_ROWS; ++r) {
@@ -215,6 +239,16 @@ __global__ void linear_small_kernel(const float* __restrict__ in, int m, int k, 
       }
     }
   }
+}
+__global__ void linear_small_kernel(const float* __restrict__ in, int m, int k, int ldi, const __nv_bfloat16* __restrict__ w,
+                                    int ldw, const float* __restrict__ bias, int n, int pre_silu, int post_silu,
+                                    float* __restrict__ out, int ldo) {
+  linear_small<false>(in, m, k, ldi, w, ldw, bias, n, pre_silu, post_silu, out, ldo);
+}
+__global__ void linear_small_f16_kernel(const float* __restrict__ in, int m, int k, int ldi, const __half* __restrict__ w,
+                                        int ldw, const float* __restrict__ bias, int n, int pre_silu, int post_silu,
+                                        float* __restrict__ out, int ldo) {
+  linear_small<true>(in, m, k, ldi, w, ldw, bias, n, pre_silu, post_silu, out, ldo);
 }
 
 // Direct convolution, one thread per output element (output channel fastest), fp32 accumulate.  Weights are [kh][kw][cin][cout]:
@@ -314,15 +348,17 @@ __global__ void pin_views_kernel(float* __restrict__ dst, int dst_ld, const floa
 }
 
 // latents [pix, cin] (fp32 or bf16) -> bf16 [repeat * pix, cpad], channels >= cin zero: the K-padded A operand of the
-// tensor-core conv_in; `repeat` = 2 duplicates the batch for classifier-free guidance ([uncond ; cond] share latents)
-template <typename TI>
+// tensor-core conv_in; `repeat` = 2 duplicates the batch for classifier-free guidance ([uncond ; cond] share latents).
+// F16: fp32 or f16 in, f16 out (fp16 models).
+template <typename TI, bool F16 = false>
 __global__ void pack_latents_kernel(const TI* __restrict__ x, long long pix, int cin, int cpad, int repeat,
-                                    __nv_bfloat16* __restrict__ out) {
+                                    typename mdb::Act<F16>::T* __restrict__ out) {
+  using A = mdb::Act<F16>;
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= pix * cpad) return;
   const long long p = i / cpad;
   const int c = static_cast<int>(i - p * cpad);
-  const __nv_bfloat16 v = (c < cin) ? __float2bfloat16_rn(ldf(x + p * cin + c)) : __float2bfloat16_rn(0.f);
+  const typename A::T v = (c < cin) ? A::from_float(ldf(x + p * cin + c)) : A::from_float(0.f);
   for (int r = 0; r < repeat; ++r) out[(r * pix + p) * cpad + c] = v;
 }
 
@@ -338,6 +374,15 @@ extern "C" int mdb_add(const void* a, const void* b, void* out, long long n, voi
   add_kernel<<<nblocks(n / 8, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const uint4*>(a), static_cast<const uint4*>(b), static_cast<uint4*>(out), n / 8);
   MDB_CHECK_LAUNCH("add_kernel");
+  return MDB_OK;
+}
+
+extern "C" int mdb_add_f16(const void* a, const void* b, void* out, long long n, void* stream) {
+  if (!a || !b || !out) return set_error(MDB_ERR_INVALID, "mdb_add_f16: null pointer");
+  if (n % 8) return set_error(MDB_ERR_UNSUPPORTED, "mdb_add_f16: n must be a multiple of 8");
+  add_f16_kernel<<<nblocks(n / 8, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const uint4*>(a), static_cast<const uint4*>(b), static_cast<uint4*>(out), n / 8);
+  MDB_CHECK_LAUNCH("add_f16_kernel");
   return MDB_OK;
 }
 
@@ -401,6 +446,19 @@ extern "C" int mdb_bf16_to_f32(const void* x, float* out, long long n, void* str
   return MDB_OK;
 }
 
+extern "C" int mdb_f32_to_f16(const float* x, void* out, long long n, void* stream) {
+  if (!x || !out) return set_error(MDB_ERR_INVALID, "mdb_f32_to_f16: null pointer");
+  f32_to_f16_kernel<<<nblocks(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(x, static_cast<__half*>(out), n);
+  MDB_CHECK_LAUNCH("f32_to_f16_kernel");
+  return MDB_OK;
+}
+extern "C" int mdb_f16_to_f32(const void* x, float* out, long long n, void* stream) {
+  if (!x || !out) return set_error(MDB_ERR_INVALID, "mdb_f16_to_f32: null pointer");
+  f16_to_f32_kernel<<<nblocks(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(static_cast<const __half*>(x), out, n);
+  MDB_CHECK_LAUNCH("f16_to_f32_kernel");
+  return MDB_OK;
+}
+
 extern "C" int mdb_timestep_embedding(const float* t, int m, int dim, int flip_sin_to_cos, float freq_shift, float* out,
                                       void* stream) {
   if (!t || !out) return set_error(MDB_ERR_INVALID, "mdb_timestep_embedding: null pointer");
@@ -417,23 +475,40 @@ extern "C" int mdb_fourier_embed(const float* x, long long rows, int d, int num_
   return MDB_OK;
 }
 
-extern "C" int mdb_linear_small(const float* in, int m, int k, int ldi, const void* w, int ldw, const float* bias, int n,
-                                int pre_silu, int post_silu, float* out, int ldo, void* stream) {
+namespace {
+template <bool F16>
+int linear_small_launch(const float* in, int m, int k, int ldi, const void* w, int ldw, const float* bias, int n, int pre_silu,
+                        int post_silu, float* out, int ldo, void* stream) {
   if (!in || !w || !out) return set_error(MDB_ERR_INVALID, "mdb_linear_small: null pointer");
   const size_t smem = sizeof(float) * LS_ROWS * k;
   if (smem > 200 * 1024) return set_error(MDB_ERR_UNSUPPORTED, "mdb_linear_small: k=%d too large", k);
+  using Elt = typename Act<F16>::T;
+  void (*kern)(const float*, int, int, int, const Elt*, int, const float*, int, int, int, float*, int);
+  if constexpr (F16) kern = linear_small_f16_kernel;
+  else kern = linear_small_kernel;
   static bool attr = false;
   if (!attr) {
-    cudaFuncSetAttribute(linear_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     attr = true;
   }
   int gy = (m + LS_ROWS - 1) / LS_ROWS;
   if (gy > 64) gy = 64;
   dim3 grid((n + 31) / 32, gy);
-  linear_small_kernel<<<grid, 256, smem, static_cast<cudaStream_t>(stream)>>>(
-      in, m, k, ldi, static_cast<const __nv_bfloat16*>(w), ldw, bias, n, pre_silu, post_silu, out, ldo);
+  kern<<<grid, 256, smem, static_cast<cudaStream_t>(stream)>>>(in, m, k, ldi, static_cast<const Elt*>(w), ldw, bias, n,
+                                                               pre_silu, post_silu, out, ldo);
   MDB_CHECK_LAUNCH("linear_small_kernel");
   return MDB_OK;
+}
+}  // namespace
+
+extern "C" int mdb_linear_small(const float* in, int m, int k, int ldi, const void* w, int ldw, const float* bias, int n,
+                                int pre_silu, int post_silu, float* out, int ldo, void* stream) {
+  return linear_small_launch<false>(in, m, k, ldi, w, ldw, bias, n, pre_silu, post_silu, out, ldo, stream);
+}
+
+extern "C" int mdb_linear_small_f16(const float* in, int m, int k, int ldi, const void* w, int ldw, const float* bias, int n,
+                                    int pre_silu, int post_silu, float* out, int ldo, void* stream) {
+  return linear_small_launch<true>(in, m, k, ldi, w, ldw, bias, n, pre_silu, post_silu, out, ldo, stream);
 }
 
 extern "C" int mdb_conv_direct(const void* x, int x_is_f32, int n, int h, int w, int cin, const float* wgt, const float* bias,
@@ -465,6 +540,21 @@ extern "C" int mdb_pack_latents(const void* x, int x_is_f32, long long pix, int 
   else
     pack_latents_kernel<__nv_bfloat16><<<nblocks(pix * cpad, 256), 256, 0, st>>>(
         static_cast<const __nv_bfloat16*>(x), pix, cin, cpad, repeat, static_cast<__nv_bfloat16*>(out));
+  MDB_CHECK_LAUNCH("pack_latents_kernel");
+  return MDB_OK;
+}
+
+extern "C" int mdb_pack_latents_f16(const void* x, int x_is_f32, long long pix, int cin, int cpad, int repeat, void* out,
+                                    void* stream) {
+  if (!x || !out) return set_error(MDB_ERR_INVALID, "mdb_pack_latents_f16: null pointer");
+  if (cpad < cin || repeat < 1) return set_error(MDB_ERR_INVALID, "mdb_pack_latents_f16: bad shape");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (x_is_f32)
+    pack_latents_kernel<float, true><<<nblocks(pix * cpad, 256), 256, 0, st>>>(static_cast<const float*>(x), pix, cin, cpad,
+                                                                               repeat, static_cast<__half*>(out));
+  else
+    pack_latents_kernel<__half, true><<<nblocks(pix * cpad, 256), 256, 0, st>>>(static_cast<const __half*>(x), pix, cin, cpad,
+                                                                                repeat, static_cast<__half*>(out));
   MDB_CHECK_LAUNCH("pack_latents_kernel");
   return MDB_OK;
 }

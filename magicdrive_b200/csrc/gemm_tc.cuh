@@ -4,7 +4,7 @@
 //
 //   D[pixel, n] = sum_{tap, c}  A[pixel shifted by tap, c] * W[n, tap*C + c]      (+ epilogue)
 //
-// * A is an NHWC bf16 activation tensor.  M tile mt is the 128 consecutive output pixels [128 mt, 128 mt + 128) of the
+// * A is an NHWC bf16 (or, for fp16 models, f16) activation tensor.  M tile mt is the 128 consecutive output pixels [128 mt, 128 mt + 128) of the
 //   flattened (image, row, column) order, whatever the image and row boundaries, so only the last tile has idle rows.
 //   - Convolutions (taps > 1, stride or padding): a 4-D (C, W, H, N) TMA map in im2col mode.  Each filter tap loads the
 //     tile's 128 pixels shifted by (s, r); the TMA walks across row and image ends, zero-fills the halo and the pixels
@@ -40,7 +40,7 @@ struct GemmParams {
   const float* bias;     // [n_out] or nullptr
   const float* rowbias;  // [n_img][rowbias_ld] or nullptr (time-embedding shift, per image)
   int rowbias_ld;
-  const __nv_bfloat16* residual;  // [pixels][ldr] or nullptr
+  const void* residual;  // bf16 (f16 in the F16 instantiations) [pixels][ldr] or nullptr
   int ldr;
   void* out;  // bf16 or fp32 [pixels][ldo]
   int ldo;
@@ -88,11 +88,13 @@ __device__ __forceinline__ float quick_gelu(float x) {
 }
 
 // Deterministic split-K finalisation: sum the fp32 partials in split order, then the same linear epilogue (+ ReLU).
-template <bool RELU = false>
+// F16: f16 residual and output (fp16 models).
+template <bool RELU = false, bool F16 = false>
 __global__ void splitk_finalize_kernel(const float* __restrict__ partial, int splits, long long pixels, int n_out,
                                        int hw_out, const float* __restrict__ bias, const float* __restrict__ rowbias,
-                                       int rowbias_ld, const __nv_bfloat16* __restrict__ residual, int ldr,
+                                       int rowbias_ld, const typename Act<F16>::T* __restrict__ residual, int ldr,
                                        void* __restrict__ out, int ldo, int out_is_f32, float out_scale) {
+  using A = Act<F16>;
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   const long long idx = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) * 4;
@@ -113,14 +115,14 @@ __global__ void splitk_finalize_kernel(const float* __restrict__ partial, int sp
   }
   for (int j = 0; j < 4; ++j) f[j] *= out_scale;
   if (residual)
-    for (int j = 0; j < 4; ++j) f[j] += __bfloat162float(residual[pix * ldr + col + j]);
+    for (int j = 0; j < 4; ++j) f[j] += A::to_float(residual[pix * ldr + col + j]);
   if constexpr (RELU)
     for (int j = 0; j < 4; ++j) f[j] = fmaxf(f[j], 0.f);
   if (out_is_f32) {
     *reinterpret_cast<float4*>(static_cast<float*>(out) + pix * ldo + col) = make_float4(f[0], f[1], f[2], f[3]);
   } else {
-    uint2 o = make_uint2(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]));
-    *reinterpret_cast<uint2*>(static_cast<__nv_bfloat16*>(out) + pix * ldo + col) = o;
+    uint2 o = make_uint2(A::pack(f[0], f[1]), A::pack(f[2], f[3]));
+    *reinterpret_cast<uint2*>(static_cast<typename A::T*>(out) + pix * ldo + col) = o;
   }
 }
 

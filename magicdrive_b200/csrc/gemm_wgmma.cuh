@@ -41,12 +41,15 @@ struct WgGemmCfg {
 
 __device__ __forceinline__ float2 ldg_f2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
 
-// RELU: the ReLU epilogue (EPI_RELU) is compiled only into its own instantiations, so the others are the plain kernel
-template <int BLOCK_N, int CTAS, bool RELU = false>
+// RELU: the ReLU epilogue (EPI_RELU) is compiled only into its own instantiations, so the others are the plain kernel.
+// F16: f16 operands, residual and output (fp16 models) in place of bf16; the accumulator and the epilogue stay fp32.
+template <int BLOCK_N, int CTAS, bool RELU = false, bool F16 = false>
 __global__ void __launch_bounds__(WgGemmCfg<BLOCK_N, CTAS>::kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                   const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   using Cfg = WgGemmCfg<BLOCK_N, CTAS>;
+  using A = Act<F16>;
+  using Elt = typename A::T;
   constexpr bool PAIR = CTAS == 2;
   constexpr int STAGES = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
@@ -163,7 +166,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
       const uint64_t adesc = make_sw128_kmajor_desc(smem_u32(smA + stage * kABytes + wg * (64 * 128)));
       const uint64_t bdesc = make_sw128_kmajor_desc(smem_u32(smB + stage * Cfg::kBBytes));
 #pragma unroll
-      for (int k = 0; k < kBlockK / 16; ++k) WgmmaSS<BLOCK_N>::run(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
+      for (int k = 0; k < kBlockK / 16; ++k) WgmmaSS<BLOCK_N, F16>::run(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
       wgmma_commit();
       wgmma_wait<1>();
       if (prev >= 0) release(prev);
@@ -221,7 +224,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
     if (p.epi_mode == EPI_GEGLU) {
       constexpr int HALF = BLOCK_N / 2;
       const int on0 = nt * HALF;
-      __nv_bfloat16* out = static_cast<__nv_bfloat16*>(p.out);
+      Elt* out = static_cast<Elt*>(p.out);
 #pragma unroll
       for (int j = 0; j < HALF / 8; ++j) {
         const int c = 8 * j + 2 * q;
@@ -236,7 +239,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
           const float a1 = fmaf(rowA[h], acc[4 * j + 2 * h + 1], fmaf(rowB[h], cv.y, bv.y * scale));
           const float g0 = fmaf(rowA[h], acc[4 * (j + HALF / 8) + 2 * h], fmaf(rowB[h], cg.x, bg.x * scale));
           const float g1 = fmaf(rowA[h], acc[4 * (j + HALF / 8) + 2 * h + 1], fmaf(rowB[h], cg.y, bg.y * scale));
-          *reinterpret_cast<uint32_t*>(out + pix[h] * p.ldo + on0 + c) = pack_bf16(a0 * gelu_erf(g0), a1 * gelu_erf(g1));
+          *reinterpret_cast<uint32_t*>(out + pix[h] * p.ldo + on0 + c) = A::pack(a0 * gelu_erf(g0), a1 * gelu_erf(g1));
         }
       }
       continue;
@@ -253,8 +256,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
           if (!ok[h]) continue;
           const float v0 = fmaf(rowA[h], acc[4 * j + 2 * h], fmaf(rowB[h], cs.x, b.x * scale));
           const float v1 = fmaf(rowA[h], acc[4 * j + 2 * h + 1], fmaf(rowB[h], cs.y, b.y * scale));
-          *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.out) + pix[h] * p.ldo + col) =
-              pack_bf16(quick_gelu(v0), quick_gelu(v1));
+          *reinterpret_cast<uint32_t*>(static_cast<Elt*>(p.out) + pix[h] * p.ldo + col) =
+              A::pack(quick_gelu(v0), quick_gelu(v1));
         }
       }
       continue;
@@ -271,8 +274,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
           if (!ok[h]) continue;
           const float v0 = fmaf(rowA[h], acc[4 * j + 2 * h], fmaf(rowB[h], cs.x, b.x * scale));
           const float v1 = fmaf(rowA[h], acc[4 * j + 2 * h + 1], fmaf(rowB[h], cs.y, b.y * scale));
-          *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.out) + pix[h] * p.ldo + col) =
-              pack_bf16(fmaxf(v0, 0.f), fmaxf(v1, 0.f));
+          *reinterpret_cast<uint32_t*>(static_cast<Elt*>(p.out) + pix[h] * p.ldo + col) =
+              A::pack(fmaxf(v0, 0.f), fmaxf(v1, 0.f));
         }
       }
       continue;
@@ -285,7 +288,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
     constexpr int RES_J = BLOCK_N == 256 ? 1 : 4;  // 256 columns of accumulators leave no registers for more
 #pragma unroll
     for (int jb = 0; jb < BLOCK_N / 8; jb += RES_J) {
-      __nv_bfloat162 res[RES_J][2];
+      typename A::T2 res[RES_J][2];
       if (p.residual) {
 #pragma unroll
         for (int jj = 0; jj < RES_J; ++jj) {
@@ -293,7 +296,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
 #pragma unroll
           for (int h = 0; h < 2; ++h)
             if (col < p.n_out && ok[h])
-              res[jj][h] = *reinterpret_cast<const __nv_bfloat162*>(p.residual + pix[h] * p.ldr + col);
+              res[jj][h] = *reinterpret_cast<const typename A::T2*>(static_cast<const Elt*>(p.residual) + pix[h] * p.ldr + col);
         }
       }
 #pragma unroll
@@ -314,16 +317,21 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constan
           float v0 = fmaf(rowA[h], acc[4 * j + 2 * h], fmaf(rowB[h], cs.x, cb.x * scale));
           float v1 = fmaf(rowA[h], acc[4 * j + 2 * h + 1], fmaf(rowB[h], cs.y, cb.y * scale));
           if (p.residual) {
-            const float2 r = __bfloat1622float2(res[jj][h]);
+            const float2 r = A::to_float2(res[jj][h]);
             v0 += r.x, v1 += r.y;
           }
           if (p.out_is_f32) {
             *reinterpret_cast<float2*>(static_cast<float*>(p.out) + pix[h] * p.ldo + col) = make_float2(v0, v1);
           } else {
-            const uint32_t pk = pack_bf16(v0, v1);
-            *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.out) + pix[h] * p.ldo + col) = pk;
+            const uint32_t pk = A::pack(v0, v1);
+            *reinterpret_cast<uint32_t*>(static_cast<Elt*>(p.out) + pix[h] * p.ldo + col) = pk;
             // the row statistics describe the values as stored: the consumer's folded LayerNorm multiplies these
-            v0 = __uint_as_float(pk << 16), v1 = __uint_as_float(pk & 0xffff0000u);
+            if constexpr (F16) {
+              const float2 sv = A::to_float2(*reinterpret_cast<const typename A::T2*>(&pk));
+              v0 = sv.x, v1 = sv.y;
+            } else {
+              v0 = __uint_as_float(pk << 16), v1 = __uint_as_float(pk & 0xffff0000u);
+            }
           }
           st_s[h] += v0 + v1;
           st_ss[h] = fmaf(v0, v0, fmaf(v1, v1, st_ss[h]));

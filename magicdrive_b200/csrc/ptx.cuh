@@ -3,6 +3,7 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -159,5 +160,30 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
   __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
   return *reinterpret_cast<uint32_t*>(&h);
 }
+__device__ __forceinline__ uint32_t pack_f16(float a, float b) {
+  __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+
+// Activation element type of a kernel instantiation: bf16, or f16 for models whose parameters are fp16.  Accumulation and
+// every epilogue stay fp32; only loads, stores and the tensor-core operands change.
+template <bool F16>
+struct Act {
+  using T = __nv_bfloat16;
+  using T2 = __nv_bfloat162;
+  static __device__ __forceinline__ uint32_t pack(float a, float b) { return pack_bf16(a, b); }
+  static __device__ __forceinline__ float2 to_float2(T2 v) { return __bfloat1622float2(v); }
+  static __device__ __forceinline__ float to_float(T v) { return __bfloat162float(v); }
+  static __device__ __forceinline__ T from_float(float v) { return __float2bfloat16_rn(v); }
+};
+template <>
+struct Act<true> {
+  using T = __half;
+  using T2 = __half2;
+  static __device__ __forceinline__ uint32_t pack(float a, float b) { return pack_f16(a, b); }
+  static __device__ __forceinline__ float2 to_float2(T2 v) { return __half22float2(v); }
+  static __device__ __forceinline__ float to_float(T v) { return __half2float(v); }
+  static __device__ __forceinline__ T from_float(float v) { return __float2half_rn(v); }
+};
 
 }  // namespace mdb

@@ -1,8 +1,8 @@
 """CUDA execution of the two hot-path networks over the C-ABI operators (magicdrive_b200.ops).
 
 Dataflow differs from the reference on purpose (GPU-first), results do not:
-  * activations are bf16 NHWC == [tokens, C]: the NCHW<->token permutes of Transformer2DModel
-    (transformer_2d.py:286,305) and the 1x1-conv / Linear distinction vanish;
+  * activations are bf16 NHWC == [tokens, C] (f16 for a UNet / ControlNet whose parameters are fp16, storage_dtype): the
+    NCHW<->token permutes of Transformer2DModel (transformer_2d.py:286,305) and the 1x1-conv / Linear distinction vanish;
   * skip-connection concats (unet_2d_blocks.py:1984,2086) are never materialised: GroupNorm and the convolutions
     read two sources;
   * self / cross-view attention use one fused QKV GEMM; cross-view attention reads the neighbours' K/V in place
@@ -17,15 +17,23 @@ from typing import Dict, List, Optional
 
 import torch
 
-from . import arch, ops
+from . import arch, f16_ops, ops
 from .params import pack_conv_weight, pack_conv_weight_k64, pack_geglu
 
-BF16, F32 = torch.bfloat16, torch.float32
+BF16, F16, F32 = torch.bfloat16, torch.float16, torch.float32
+
+
+def storage_dtype(sd: Dict[str, torch.Tensor]) -> torch.dtype:
+    """Activation and weight storage of a UNet / ControlNet engine: f16 when every floating tensor of the module is fp16
+    (from_pretrained(torch_dtype=torch.float16), .to(torch.float16): the precision the reference's inference runs), bf16
+    for any other parameter dtype.  The VAE, CLIP and Inception engines are bf16 whatever their parameters."""
+    fl = [v.dtype for v in sd.values() if v.is_floating_point()]
+    return F16 if fl and all(d == F16 for d in fl) else BF16
 
 
 @dataclass
 class FMap:
-    """A feature map: data is [n*h*w, c] bf16 (NHWC)."""
+    """A feature map: data is [n*h*w, c] bf16 or f16 (NHWC)."""
     data: torch.Tensor
     n: int
     h: int
@@ -42,22 +50,28 @@ def _f32(t):
 
 
 class _Weights:
-    """Packs a reference state dict into kernel-ready device tensors (bf16 K-major matrices, fp32 biases)."""
+    """Packs a reference state dict into kernel-ready device tensors (bf16 or f16 K-major matrices, fp32 biases)."""
 
     fold_dtype = BF16  # storage of weights that are PRODUCTS of checkpoint tensors (W * gamma); the CPU host-logic tests
     #                    set fp32 so that the fold's algebra is checked to 1e-5, apart from its bf16 rounding
 
-    def __init__(self, sd: Dict[str, torch.Tensor], device):
+    def __init__(self, sd: Dict[str, torch.Tensor], device, dtype=BF16):
         self.sd = sd
         self.device = device
+        self.dtype = dtype  # storage of the weight matrices: bf16, or f16 for an fp16 module
+        if dtype == F16:
+            self.fold_dtype = F16
         self.t: Dict[str, torch.Tensor] = {}
+
+    def _st(self, t):
+        return t.detach().to(dtype=self.dtype).contiguous()
 
     def raw(self, key):
         return self.sd[key].detach().to(self.device)
 
     def conv(self, p):
         if p + ".w" not in self.t:
-            self.t[p + ".w"] = pack_conv_weight(self.raw(p + ".weight").float())
+            self.t[p + ".w"] = pack_conv_weight(self.raw(p + ".weight").float(), self.dtype)
             self.t[p + ".b"] = _f32(self.raw(p + ".bias"))
         return self.t[p + ".w"], self.t[p + ".b"]
 
@@ -73,7 +87,7 @@ class _Weights:
             w = self.raw(p + ".weight").float()
             wp = torch.zeros((w.shape[0], cpad, w.shape[2], w.shape[3]), dtype=F32, device=w.device)
             wp[:, : w.shape[1]] = w
-            self.t[p + ".wk"] = pack_conv_weight(wp)
+            self.t[p + ".wk"] = pack_conv_weight(wp, self.dtype)
             self.t[p + ".b"] = _f32(self.raw(p + ".bias"))
         return self.t[p + ".wk"], self.t[p + ".b"]
 
@@ -85,13 +99,13 @@ class _Weights:
             wp[: w.shape[0]] = w
             bp = torch.zeros((npad,), dtype=F32, device=w.device)
             bp[: w.shape[0]] = self.raw(p + ".bias").float()
-            self.t[p + ".wn"] = pack_conv_weight(wp)
+            self.t[p + ".wn"] = pack_conv_weight(wp, self.dtype)
             self.t[p + ".bn"] = bp
         return self.t[p + ".wn"], self.t[p + ".bn"]
 
     def lin(self, p, bias=True):
         if p + ".w" not in self.t:
-            self.t[p + ".w"] = _bf(self.raw(p + ".weight"))
+            self.t[p + ".w"] = self._st(self.raw(p + ".weight"))
             self.t[p + ".b"] = _f32(self.raw(p + ".bias")) if bias else None
         return self.t[p + ".w"], self.t[p + ".b"]
 
@@ -103,18 +117,18 @@ class _Weights:
 
     def cat_lin(self, name, prefixes, suffix=".weight"):
         if name not in self.t:
-            self.t[name] = _bf(torch.cat([self.raw(p + suffix) for p in prefixes], 0))
+            self.t[name] = self._st(torch.cat([self.raw(p + suffix) for p in prefixes], 0))
         return self.t[name]
 
     def geglu(self, p):
         if p + ".gw" not in self.t:
-            w, b = pack_geglu(self.raw(p + ".weight").float(), self.raw(p + ".bias").float())
+            w, b = pack_geglu(self.raw(p + ".weight").float(), self.raw(p + ".bias").float(), dtype=self.dtype)
             self.t[p + ".gw"], self.t[p + ".gb"] = w, b
         return self.t[p + ".gw"], self.t[p + ".gb"]
 
     def ln_lin(self, name, norm, prefixes, geglu=False):
         """LayerNorm `norm` folded into the linear(s) `prefixes` that consume it (mdb_gemm_desc.ln_*):
-        W' = W * gamma (bf16), c = W beta + b (fp32), colsum_n = sum_k W'[n, k] (of the rounded W', fp32).
+        W' = W * gamma (fold_dtype), c = W beta + b (fp32), colsum_n = sum_k W'[n, k] (of the rounded W', fp32).
         Returns (W', c, colsum); with geglu the three are re-ordered to the kernel's [128 value | 128 gate] tiles."""
         if name + ".w" not in self.t:
             w = torch.cat([self.raw(p + ".weight").float() for p in prefixes], 0)
@@ -140,7 +154,7 @@ class _Weights:
             bo = self.raw(blk + ".attn4.to_out.0.bias").float()
             wc = self.raw(blk + ".connector.weight").float()
             bc = self.raw(blk + ".connector.bias").float()
-            self.t[k + ".w"] = _bf(wc @ wo)
+            self.t[k + ".w"] = self._st(wc @ wo)
             self.t[k + ".b"] = _f32(float(bias_count) * (wc @ bo) + bc)
         return self.t[k + ".w"], self.t[k + ".b"]
 
@@ -176,7 +190,8 @@ class _Net:
 
     def __init__(self, cfg, sd, device, multiview: bool):
         self.cfg = cfg
-        self.W = _Weights(sd, device)
+        self.dtype = storage_dtype(sd)  # activations and tensor-core operands: bf16, or f16 for an fp16 module
+        self.W = _Weights(sd, device, self.dtype)
         self.device = device
         self.multiview = multiview
         self.down = arch.down_blocks(cfg, multiview)
@@ -306,7 +321,7 @@ class _Net:
 
     def context_kv(self, ctx_bf16: torch.Tensor) -> Dict[str, torch.Tensor]:
         """attn2 K/V projections of the conditioning tokens for every transformer (step-invariant).
-        ctx: [V*Lc, 768] bf16 -> {prefix: [V*Lc, 2C] bf16}."""
+        ctx: [V*Lc, 768] in the storage type (models.cast_as) -> {prefix: [V*Lc, 2C]}."""
         out = {}
         for tr in self.transformers:
             blk = tr.prefix + ".transformer_blocks.0"
@@ -459,7 +474,8 @@ class _Net:
     CIN_PAD = 64  # latent channels are zero-padded to one 64-wide K block so conv_in runs on the tensor-core path
 
     def conv_in(self, x_pad: torch.Tensor, n, h, w, residual=None) -> FMap:
-        """x_pad: [n*h*w, 64] bf16 (ops.pack_latents); optional residual [n*h*w, C0] (the BEV-map embedding)."""
+        """x_pad: [n*h*w, 64] in the storage type (models.pack_latents_as); optional residual [n*h*w, C0] (the BEV-map
+        embedding)."""
         wk, b = self.W.conv_k_padded("conv_in", self.CIN_PAD)
         c0 = self.cfg.block_out_channels[0]
         out = ops.gemm_conv(x_pad, wk, n_img=n, h_in=h, w_in=w, c0=self.CIN_PAD, lda0=self.CIN_PAD, n_out=c0, taps=3,
@@ -586,7 +602,9 @@ class ControlNetEngine(_Net):
         return ctx.reshape(b * n_cam, ctx.shape[2], ctx.shape[3]).contiguous()
 
     def map_embedding(self, cond: torch.Tensor) -> torch.Tensor:
-        """BEV map (b, 8, H, W) -> [b, h, w, 320] bf16 NHWC, once per scene (map_embedder.py:66-76)."""
+        """BEV map (b, 8, H, W) -> [b, h, w, 320] NHWC in the storage type, once per scene (map_embedder.py:66-76).  The
+        encoder runs on the fp32-weight direct-convolution kernels either way; for an f16 engine its fp32 output is
+        rounded to f16."""
         x = cond.to(self.device, F32).permute(0, 2, 3, 1).contiguous()
         n, h, w = x.shape[0], x.shape[1], x.shape[2]
         layers = arch.map_encoder_layers(self.cfg)
@@ -599,9 +617,9 @@ class ControlNetEngine(_Net):
                 x = ops.adaptive_avgpool(x, n, h, w, ci, ho, wo, silu=True)
                 h, w = ho, wo
             x = ops.conv_direct(x, wd, bias, n=n, h=h, w=w, cin=ci, cout=co, k=3, stride=stride, pad=pad, silu=not last,
-                                out_f32=not last)
+                                out_f32=not last or self.dtype == F16)
             h, w = x.shape[1], x.shape[2]
-        return x  # bf16 [b, h, w, 320]
+        return f16_ops.f32_to_f16(x) if self.dtype == F16 else x  # [b, h, w, 320]
 
     # ---------------------------------------------------------------- per-step
     def forward(self, latents_pad, n, h, w, t_f32, ctx_kv, lc, map_emb_per_view: torch.Tensor,

@@ -18,10 +18,37 @@ from typing import Any, Dict, List, Tuple, Union
 import torch
 import torch.nn as nn
 
-from . import arch, ops
-from .engine import ControlNetEngine, InceptionEngine, TextEncoderEngine, UNetEngine, VaeDecoderEngine, VaeEncoderEngine
+from . import arch, f16_ops, ops
+from .engine import (ControlNetEngine, InceptionEngine, TextEncoderEngine, UNetEngine, VaeDecoderEngine, VaeEncoderEngine,
+                     storage_dtype)
 
-BF16, F32 = torch.bfloat16, torch.float32
+BF16, F16, F32 = torch.bfloat16, torch.float16, torch.float32
+
+
+def _nhwc(st, x):
+    """NCHW tensor -> [n*h*w, c] in the storage type `st`: mdb_nchw_to_nhwc for bf16 engines; for f16 engines a layout
+    copy at the module boundary (the denoiser keeps its latents NHWC and never takes this path)."""
+    if st == BF16:
+        return ops.nchw_to_nhwc(x)
+    n, c, h, w = x.shape
+    return x.permute(0, 2, 3, 1).reshape(n * h * w, c).to(F16).contiguous()
+
+
+def _nchw(st, x, n, c, h, w, dtype):
+    """[n*h*w, >= c] in the storage type `st` -> NCHW `dtype` (the inverse of _nhwc)."""
+    if st == BF16:
+        return ops.nhwc_to_nchw(x, n, c, h, w, F32).to(dtype)
+    return x.reshape(n, h, w, -1)[..., :c].permute(0, 3, 1, 2).to(dtype).contiguous()
+
+
+def pack_latents_as(st, x, cpad, repeat=1):
+    """Latents [pix, c] -> conv_in's channel-padded operand in the storage type `st`."""
+    return (f16_ops.pack_latents_f16 if st == F16 else ops.pack_latents)(x, cpad, repeat=repeat)
+
+
+def cast_as(st, ctx_f32):
+    """fp32 conditioning tokens -> the storage type `st` (the input of the engines' context_kv)."""
+    return f16_ops.f32_to_f16(ctx_f32) if st == F16 else ops.f32_to_bf16(ctx_f32)
 
 
 @dataclass
@@ -83,6 +110,13 @@ class _B200Module(nn.Module):
     @property
     def device(self):
         return next(self.parameters()).device
+
+    def storage_dtype(self) -> torch.dtype:
+        """The storage type its UNet / ControlNet engine computes in (engine.storage_dtype): f16 for fp16 parameters."""
+        st = self._ctx_cache.get("storage")  # dropped with the engine whenever parameters change
+        if st is None:
+            st = self._ctx_cache["storage"] = storage_dtype(self.state_dict())
+        return st
 
     def set_use_memory_efficient_attention_xformers(self, *a, **k):  # attention is always our fused kernel
         return None
@@ -192,7 +226,8 @@ class UNet2DConditionModelMultiview(_B200Module):
         return self._get_engine(UNetEngine)
 
     def prepare_context(self, encoder_hidden_states: torch.Tensor):
-        """Project the conditioning tokens to K/V for all 16 transformer blocks (cached while the tensor is unchanged)."""
+        """Project the conditioning tokens to K/V for all 16 transformer blocks (cached while the tensor is unchanged).
+        Tokens in the engine's storage type are used as they are, any other dtype is rounded to it."""
         eng = self._get_engine(UNetEngine)
         key = (encoder_hidden_states.data_ptr(), encoder_hidden_states._version, tuple(encoder_hidden_states.shape),
                encoder_hidden_states.dtype)
@@ -200,7 +235,8 @@ class UNet2DConditionModelMultiview(_B200Module):
         if hit is None or hit[0] != key:
             v, lc, cdim = encoder_hidden_states.shape
             ctx = encoder_hidden_states.reshape(v * lc, cdim)
-            ctx = ops.f32_to_bf16(ctx.float().contiguous()) if ctx.dtype != BF16 else ctx.contiguous()
+            st = self.storage_dtype()
+            ctx = ctx.contiguous() if ctx.dtype == st else cast_as(st, ctx.float().contiguous())
             hit = (key, eng.context_kv(ctx), lc, encoder_hidden_states)  # keep a ref so data_ptr is not recycled
             self._ctx_cache["kv"] = hit
         return hit[1], hit[2]
@@ -216,13 +252,14 @@ class UNet2DConditionModelMultiview(_B200Module):
         if self.arch_cfg.multiview and n % self.arch_cfg.n_cam:
             raise ValueError(f"batch {n} is not a multiple of the {self.arch_cfg.n_cam} camera views")
         ctx_kv, lc = self.prepare_context(encoder_hidden_states)
-        x = ops.pack_latents(ops.nchw_to_nhwc(sample), UNetEngine.CIN_PAD)
+        st = self.storage_dtype()
+        x = pack_latents_as(st, _nhwc(st, sample), UNetEngine.CIN_PAD)
         t = _timesteps_f32(timestep, n, sample.device)
         down = mid = None
         if down_block_additional_residuals is not None:
-            down = [ops.nchw_to_nhwc(r) for r in down_block_additional_residuals]
+            down = [_nhwc(st, r) for r in down_block_additional_residuals]
         if mid_block_additional_residual is not None:
-            mid = ops.nchw_to_nhwc(mid_block_additional_residual)
+            mid = _nhwc(st, mid_block_additional_residual)
         eps = eng.forward(x, n, h, w, t, ctx_kv, lc, down, mid)  # fp32 [n*h*w, 8], first out_channels valid
         co = self.arch_cfg.out_channels
         out = eps[:, :co].reshape(n, h, w, co).permute(0, 3, 1, 2).contiguous().to(sample.dtype)
@@ -368,8 +405,7 @@ class BEVControlNetModel(_B200Module):
         if hit is None or hit[0] != key:
             n_cam = camera_param.shape[1]
             ctx = eng.context(camera_param, bboxes_3d_data, encoder_hidden_states)  # fp32 (V, Lc, 768)
-            ctx_bf = ops.f32_to_bf16(ctx.reshape(-1, ctx.shape[-1]))
-            kv = eng.context_kv(ctx_bf)
+            kv = eng.context_kv(cast_as(self.storage_dtype(), ctx.reshape(-1, ctx.shape[-1])))
             memb = eng.map_embedding(controlnet_cond)  # [b, h, w, 320]
             memb = memb.repeat_interleave(n_cam, dim=0).contiguous()  # 'b ... -> (b repeat) ...' (:842-843)
             hit = (key, dict(ctx=ctx, kv=kv, lc=ctx.shape[1], map=memb),
@@ -390,7 +426,8 @@ class BEVControlNetModel(_B200Module):
         eng = self._get_engine(ControlNetEngine)
         b, n_cam, c, h, w = sample.shape
         cond = self.prepare_conditions(camera_param, bboxes_3d_data, encoder_hidden_states, controlnet_cond)
-        x = ops.pack_latents(ops.nchw_to_nhwc(sample.reshape(b * n_cam, c, h, w)), ControlNetEngine.CIN_PAD)
+        st = self.storage_dtype()
+        x = pack_latents_as(st, _nhwc(st, sample.reshape(b * n_cam, c, h, w)), ControlNetEngine.CIN_PAD)
         t = _timesteps_f32(timestep, b, sample.device)
         if t.numel() == b and n_cam > 1:
             t = t.repeat_interleave(n_cam)  # 'b ... -> (b repeat) ...' (:840-841)
@@ -399,8 +436,8 @@ class BEVControlNetModel(_B200Module):
                  else float(conditioning_scale))
         down, mid, skips, xm = eng.forward(x, b * n_cam, h, w, t, cond["kv"], cond["lc"], cond["map"], scale)
         dt = sample.dtype
-        down_nchw = [ops.nhwc_to_nchw(d, s.n, s.c, s.h, s.w, F32).to(dt) for d, s in zip(down, skips)]
-        mid_nchw = ops.nhwc_to_nchw(mid, xm.n, xm.c, xm.h, xm.w, F32).to(dt)
+        down_nchw = [_nchw(st, d, s.n, s.c, s.h, s.w, dt) for d, s in zip(down, skips)]
+        mid_nchw = _nchw(st, mid, xm.n, xm.c, xm.h, xm.w, dt)
         ctx = cond["ctx"].to(dt)
         if not return_dict:
             return (down_nchw, mid_nchw, ctx)

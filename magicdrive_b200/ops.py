@@ -2,7 +2,10 @@
 
 torch is plumbing only: it owns device memory and the CUDA stream; every function here forwards raw pointers to
 `libmagicdrive_b200.so` and raises if the library / a CUDA device is unavailable (no CPU or eager fallback).
-Feature maps are NHWC bf16 ("channels innermost") everywhere; a token matrix [tokens, C] is the same layout.
+Feature maps are NHWC bf16 ("channels innermost") everywhere; a token matrix [tokens, C] is the same layout.  The operators of
+the denoising step (gemm_conv, groupnorm, attention, add, upsample_nearest, linear_small's weights) also take f16 tensors --
+the engines of models with fp16 parameters -- and then run their f16 kernels: the element type follows the tensors passed in.
+The operators that only fp16 models need (fp32 <-> f16 conversion, f16 latent packing) are in f16_ops.py.
 
 One process drives ONE device (the launch contract: one process per GPU): the module-level workspace slot / launch counter and the
 library's cached device attributes (SM count, per-kernel shared-memory opt-ins) are per process, not per device, and not thread-safe.
@@ -18,6 +21,7 @@ from . import _lib
 from ._lib import GemmDesc, check
 
 BF16 = torch.bfloat16
+F16 = torch.float16
 F32 = torch.float32
 
 GEMM_VARIANT = int(os.environ.get('MDB_GEMM_VARIANT', '0'))  # A/B hook: mdb_gemm_desc.kernel_variant (2 = single CTAs, 3 = CTA pairs)
@@ -129,7 +133,8 @@ def gemm_conv(a0: torch.Tensor, w: torch.Tensor, *, n_img: int, h_in: int, w_in:
               emit_stats: bool = False, quick_gelu: bool = False, relu: bool = False, taps_h: Optional[int] = None,
               taps_w: Optional[int] = None, pad_h: Optional[int] = None, pad_w: Optional[int] = None,
               pad_h_end: int = 0, pad_w_end: int = 0):
-    """wgmma GEMM / implicit-GEMM conv (mdb_gemm_conv).  `a0` (and `a1`) are NHWC bf16 buffers whose pixel
+    """wgmma GEMM / implicit-GEMM conv (mdb_gemm_conv).  `a0` (and `a1`) are NHWC bf16 (or f16, then `w`, `residual` and
+    the output are f16 too) buffers whose pixel
     stride is lda* elements; `w` is bf16 [n_out, taps_h*taps_w*K64] with K64 = c0+c1, each rounded up to 64
     (params.pack_conv_weight_k64; the plain (tap, channel) layout when c0 and c1 are multiples of 64).
     `taps` / `pad` give a square filter; taps_h, taps_w, pad_h, pad_w override them per dimension (1x7, 7x1, ...).
@@ -141,6 +146,10 @@ def gemm_conv(a0: torch.Tensor, w: torch.Tensor, *, n_img: int, h_in: int, w_in:
     output rows -> (out, RowStats).  quick_gelu: out = y * sigmoid(1.702 y) (CLIP's MLP activation)."""
     global _launches
     _need_cuda(a0, w)
+    act = F16 if a0.dtype == F16 else BF16  # mdb_gemm_desc.operand_dtype: a0, a1, w and residual share it
+    if act == F16:
+        assert w.dtype == F16 and (a1 is None or a1.dtype == F16) and (residual is None or residual.dtype == F16), \
+            "an f16 gemm_conv takes f16 weights, second source and residual"
     th = taps if taps_h is None else taps_h
     tw = taps if taps_w is None else taps_w
     ph = pad if pad_h is None else pad_h
@@ -152,7 +161,7 @@ def gemm_conv(a0: torch.Tensor, w: torch.Tensor, *, n_img: int, h_in: int, w_in:
     pixels = n_img * h_out * w_out
     width = n_out // 2 if geglu else n_out
     if out is None:
-        out = torch.empty((pixels, width), dtype=F32 if out_f32 else BF16, device=a0.device)
+        out = torch.empty((pixels, width), dtype=F32 if out_f32 else act, device=a0.device)
         ldo = width
     elif ldo is None:
         ldo = out.stride(0) if out.dim() == 2 else out.shape[-1]
@@ -178,6 +187,7 @@ def gemm_conv(a0: torch.Tensor, w: torch.Tensor, *, n_img: int, h_in: int, w_in:
         d.workspace, d.workspace_bytes = None, 0
     d.force_block_n, d.force_splits = force_block_n, force_splits
     d.kernel_variant = kernel_variant or GEMM_VARIANT
+    d.operand_dtype = int(act == F16)
     L = _lib.lib()
     if ln is not None:
         d.ln_stats, d.ln_parts, d.ln_eps, d.ln_colsum = ln.data.data_ptr(), ln.parts, float(ln_eps), _ptr(ln_colsum)
@@ -240,10 +250,12 @@ def conv_direct(x, wgt, bias, *, n, h, w, cin, cout, k, stride=(1, 1), pad=(1, 1
 def groupnorm(x0, c0, ld0, n_img, hw, gamma, beta, eps, silu, x1=None, c1=0, ld1=0, groups=32):
     global _launches
     _need_cuda(x0)
-    out = torch.empty((n_img * hw, c0 + c1), dtype=BF16, device=x0.device)
+    f16 = x0.dtype == F16  # mdb_groupnorm_f16: f16 sources and output
+    out = torch.empty((n_img * hw, c0 + c1), dtype=F16 if f16 else BF16, device=x0.device)
     stats = torch.empty((max(n_img, 160) * groups * 2,), dtype=F32, device=x0.device)  # scratch: per-(image | CTA run) group partials
-    check(_lib.lib().mdb_groupnorm(_ptr(x0), c0, ld0, _ptr(x1), c1, ld1, n_img, hw, groups, float(eps), _ptr(gamma),
-                                   _ptr(beta), int(silu), _ptr(out), c0 + c1, _ptr(stats), _stream()), "mdb_groupnorm")
+    fn = _lib.lib().mdb_groupnorm_f16 if f16 else _lib.lib().mdb_groupnorm
+    check(fn(_ptr(x0), c0, ld0, _ptr(x1), c1, ld1, n_img, hw, groups, float(eps), _ptr(gamma), _ptr(beta), int(silu), _ptr(out),
+             c0 + c1, _ptr(stats), _stream()), "mdb_groupnorm")
     _launches += 2 if os.environ.get("MDB_GN_TWO_KERNEL") else 1  # one fused kernel (A/B: stats + apply)
     return out
 
@@ -274,8 +286,8 @@ def attention(q, k, v, *, b, heads, lq, lk, d, ldq, ldk, ldv, scale, kv_index=No
               kv_len=None):
     """q: [b*lq, >=heads*d] view with row stride ldq, k/v [b_kv*lk, ...] likewise; returns [b*lq, heads*d] bf16.
     kv_index: int32 [b, n_sets] (n_sets <= 8), -1 = empty slot; the sets' outputs are summed.  kv_len: int32 [b] keys per
-    query batch (mdb_attention_varlen), None = lk."""
-    if kv_len is not None:
+    query batch (mdb_attention_varlen), None = lk.  f16 q/k/v (an fp16 model) give an f16 output (mdb_attention_varlen_f16)."""
+    if kv_len is not None or q.dtype == F16:
         return attention_multi(q, [(k, v, ldk, b if b_kv is None else b_kv, ldv)], b=b, heads=heads, lq=lq, lk=lk, d=d,
                                ldq=ldq, scale=scale, kv_index=kv_index, n_sets=n_sets, out=out, kv_len=kv_len)
     b_kv = b if b_kv is None else b_kv
@@ -299,15 +311,21 @@ def attention_multi(q, sources, *, b, heads, lq, lk, d, ldq, scale, kv_index, n_
     global _launches
     _need_cuda(q, *[t for s_ in sources for t in s_[:2]], kv_len)
     n = len(sources)
+    f16 = q.dtype == F16  # mdb_attention_varlen_f16 (kv_len may be None there)
     if out is None:
-        out = torch.empty((b * lq, heads * d), dtype=BF16, device=q.device)
+        out = torch.empty((b * lq, heads * d), dtype=F16 if f16 else BF16, device=q.device)
     ks = (C.c_void_p * n)(*[s_[0].data_ptr() for s_ in sources])
     vs = (C.c_void_p * n)(*[s_[1].data_ptr() for s_ in sources])
     ldk = (C.c_int * n)(*[int(s_[2]) for s_ in sources])
     ldv = (C.c_int * n)(*[int(s_[4] if len(s_) > 4 else s_[2]) for s_ in sources])
     bkv = (C.c_int * n)(*[int(s_[3]) for s_ in sources])
     e0 = _prof_begin()
-    if kv_len is None:
+    if f16:
+        assert kv_len is None or (kv_len.dtype == torch.int32 and kv_len.numel() == b)
+        check(_lib.lib().mdb_attention_varlen_f16(_ptr(q), ldq, n, ks, ldk, vs, ldv, bkv, _ptr(out), out.stride(0), b, heads, lq,
+                                                  lk, d, _ptr(kv_index), n_sets, _ptr(kv_len), float(scale), _stream()),
+              "mdb_attention_varlen_f16")
+    elif kv_len is None:
         check(_lib.lib().mdb_attention_multi(_ptr(q), ldq, n, ks, ldk, vs, ldv, bkv, _ptr(out), out.stride(0), b, heads, lq, lk,
                                              d, _ptr(kv_index), n_sets, float(scale), _stream()), "mdb_attention_multi")
     else:
@@ -366,7 +384,8 @@ def add(a, b):
     global _launches
     _need_cuda(a, b)
     out = torch.empty_like(a)
-    check(_lib.lib().mdb_add(_ptr(a), _ptr(b), _ptr(out), a.numel(), _stream()), "mdb_add")
+    fn = _lib.lib().mdb_add_f16 if a.dtype == F16 else _lib.lib().mdb_add  # f16 a and b: mdb_add_f16
+    check(fn(_ptr(a), _ptr(b), _ptr(out), a.numel(), _stream()), "mdb_add")
     _launches += 1
     return out
 
@@ -374,7 +393,8 @@ def add(a, b):
 def upsample_nearest(x, n, h, w, c, ho, wo):
     global _launches
     _need_cuda(x)
-    out = torch.empty((n * ho * wo, c), dtype=BF16, device=x.device)
+    # the kernel copies 2-byte elements: an f16 map gives an f16 output
+    out = torch.empty((n * ho * wo, c), dtype=F16 if x.dtype == F16 else BF16, device=x.device)
     check(_lib.lib().mdb_upsample_nearest(_ptr(x), n, h, w, c, _ptr(out), ho, wo, _stream()), "mdb_upsample_nearest")
     _launches += 1
     return out
@@ -437,14 +457,15 @@ def fid_input(x, *, nhwc: bool, quantize: bool, normalize: bool, size=None):
 
 
 def linear_small(x, w, bias=None, pre_silu=False, post_silu=False):
-    """x fp32 [m, k]; w bf16 [n, k]; returns fp32 [m, n]."""
+    """x fp32 [m, k]; w bf16 (or f16: mdb_linear_small_f16) [n, k]; returns fp32 [m, n]."""
     global _launches
     _need_cuda(x, w)
     m, k = x.shape
     n = w.shape[0]
     out = torch.empty((m, n), dtype=F32, device=x.device)
-    check(_lib.lib().mdb_linear_small(_ptr(x), m, k, x.stride(0), _ptr(w), w.stride(0), _ptr(bias), n, int(pre_silu),
-                                      int(post_silu), _ptr(out), n, _stream()), "mdb_linear_small")
+    fn = _lib.lib().mdb_linear_small_f16 if w.dtype == F16 else _lib.lib().mdb_linear_small
+    check(fn(_ptr(x), m, k, x.stride(0), _ptr(w), w.stride(0), _ptr(bias), n, int(pre_silu), int(post_silu), _ptr(out), n,
+             _stream()), "mdb_linear_small")
     _launches += 1
     return out
 

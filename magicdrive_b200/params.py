@@ -2,10 +2,10 @@
 import torch
 
 
-def pack_conv_weight(w: torch.Tensor) -> torch.Tensor:
-    """[Cout, Cin, kh, kw] -> bf16 [Cout, kh*kw*Cin] with K ordered (tap, channel) as mdb_gemm_conv expects."""
+def pack_conv_weight(w: torch.Tensor, dtype=torch.bfloat16) -> torch.Tensor:
+    """[Cout, Cin, kh, kw] -> bf16 (or `dtype`) [Cout, kh*kw*Cin] with K ordered (tap, channel) as mdb_gemm_conv expects."""
     co, ci, kh, kw = w.shape
-    return w.permute(0, 2, 3, 1).reshape(co, kh * kw * ci).contiguous().to(torch.bfloat16)
+    return w.permute(0, 2, 3, 1).reshape(co, kh * kw * ci).contiguous().to(dtype)
 
 
 def pack_conv_weight_k64(w: torch.Tensor, splits=None, dtype=torch.bfloat16) -> torch.Tensor:

@@ -20,7 +20,7 @@ import torch
 
 from . import ops
 from .engine import CtxLen, FMap
-from .models import BEVControlNetModel, UNet2DConditionModelMultiview
+from .models import BEVControlNetModel, UNet2DConditionModelMultiview, cast_as, pack_latents_as
 
 F32, BF16 = torch.float32, torch.bfloat16
 
@@ -163,6 +163,8 @@ class BEVControlNetDenoiser:
             raise ValueError("box_capacity is not implemented for view-sharded runs (view_shard=)")
         self.box_capacity = None if box_capacity is None else int(box_capacity)
         self.unet, self.controlnet, self.vae = unet, controlnet, vae
+        self.view_shard = view_shard
+        self._check_dtypes(unet.storage_dtype(), controlnet.storage_dtype())
         self.text_encoder, self.tokenizer = text_encoder, tokenizer
         self.overlap_controlnet = overlap_controlnet
         # programmatic dependent launch on the single-stream UNet up path (A/B switch until measured: MDB_PDL_DECODER=1)
@@ -171,7 +173,6 @@ class BEVControlNetDenoiser:
         # ControlNet residual additions ride the zero convolutions' epilogues (MDB_FUSE_RESIDUAL_ADDS=0: the separate
         # additions of round 1, kept as the A/B and as the path the sharded mode's halves use)
         self.fuse_residual_adds = os.environ.get("MDB_FUSE_RESIDUAL_ADDS", "1") == "1"
-        self.view_shard = view_shard
         unet.set_view_shard(view_shard)
         self._side = {}
         self.generator = None  # optional torch.Generator for latents=None calls
@@ -184,6 +185,16 @@ class BEVControlNetDenoiser:
         self._cond_graph = None        # CUDA graph of _encode_conditions on the resident state
         self._cond_graph_state = None
         self._static = None
+
+    def _check_dtypes(self, du, dc):
+        """du, dc: the storage types of the UNet and the ControlNet (their storage_dtype()).  They share the step's
+        activations, so both compute in fp16 or neither does; fp16 runs on one GPU: the view-sharded mode stays bf16."""
+        fu, fc = du == torch.float16, dc == torch.float16
+        if fu != fc:
+            raise ValueError("the UNet and the ControlNet must both have fp16 parameters or neither (got "
+                             f"{self.unet.dtype} and {self.controlnet.dtype})")
+        if fu and self.view_shard is not None:
+            raise ValueError("fp16 models are not implemented for view-sharded runs (view_shard=)")
 
     def release_graph(self):
         """Drop the captured CUDA graphs (they are re-captured on the next use)."""
@@ -247,7 +258,7 @@ class BEVControlNetDenoiser:
         ue, ce = st["ue"], st["ce"]
         V, h, w, lc = st["V"], st["h"], st["w"], st["lc"]
         vh, npix = V // 2, lat.shape[0]
-        x = ops.pack_latents(lat, ue.CIN_PAD, repeat=1)  # both halves read the same latents (:352-354)
+        x = pack_latents_as(st["act"], lat, ue.CIN_PAD, repeat=1)  # both halves read the same latents (:352-354)
         if "eps_buf" not in st:
             st["eps_buf"] = torch.zeros((2 * npix, ue.COUT_PAD), dtype=F32, device=lat.device)
         eps = st["eps_buf"]
@@ -281,8 +292,8 @@ class BEVControlNetDenoiser:
         """ControlNet + UNet on the whole guidance batch; returns eps fp32 [V*h*w, 8]."""
         ue, ce = st["ue"], st["ce"]
         V, h, w = st["V"], st["h"], st["w"]
-        # bf16, channel-padded to one K block; CFG: [uncond ; cond] share the latents (:352-354) -> repeat = 2
-        x = ops.pack_latents(lat, ue.CIN_PAD, repeat=st["dup"])
+        # bf16 (f16 for fp16 models), channel-padded to one K block; CFG: [uncond ; cond] share the latents (:352-354) -> repeat = 2
+        x = pack_latents_as(st["act"], lat, ue.CIN_PAD, repeat=st["dup"])
         if self.overlap_controlnet and st.get("u_temb") is not None:
             # The ControlNet and the UNet's down/mid path only meet at the skip additions: run them on two streams so
             # that each one's small-grid kernels and per-kernel tails are filled by the other (captured as two branches
@@ -340,8 +351,9 @@ class BEVControlNetDenoiser:
         """Host -> device staging + all step-invariant work.  latents: (S, 4, h, w) initial noise shared by the views
         (:326) or (S, n_cam, 4, h, w).  conditional_latents: list[S] of list[n_cam] of clean (4, h, w) latents or None
         (StableDiffusionBEVControlNetGivenViewPipeline, pipeline_bev_controlnet_given_view.py:36-37)."""
-        dev = self.unet.device
         cn, un = self.controlnet, self.unet
+        self._check_dtypes(un.storage_dtype(), cn.storage_dtype())  # the modules may have changed dtype since
+        dev = self.unet.device
         if camera_param is None:
             # the reference falls back to the learned null camera and switches guidance off (pipeline_bev_controlnet.py:
             # 330-338): there is no conditional camera to guide towards
@@ -460,7 +472,8 @@ class BEVControlNetDenoiser:
                 self._encode_conditions(st)
             return st
         dev_in = {k: v.to(dev) for k, v in inputs.items()}
-        st = dict(ue=un.engine(), ce=cn.engine(), V=V, h=h, w=w, S=S, n_cam=n_cam, cfg=cfg, dup=dup, sig=sig, inputs=dev_in,
+        st = dict(ue=un.engine(), ce=cn.engine(), act=un.storage_dtype(), V=V, h=h, w=w, S=S, n_cam=n_cam, cfg=cfg, dup=dup,
+                  sig=sig, inputs=dev_in,
                   guidance=float(guidance_scale), cond_scale=float(controlnet_conditioning_scale), latents=dev_in["latents"],
                   lc=lc, c_kv=None, u_kv=None, map=None,
                   t_dev=torch.zeros(V, dtype=F32, device=dev),
@@ -494,8 +507,8 @@ class BEVControlNetDenoiser:
         boxes = None if "bboxes" not in x else dict(bboxes=x["bboxes"], classes=x["classes"], masks=x["masks"])
         ctx = ce.context(x["camera"], boxes, x["text"])  # fp32 (V, Lc, 768)
         assert ctx.shape[1] == st["lc"], (ctx.shape, st["lc"])
-        ctx_bf = ops.f32_to_bf16(ctx.reshape(-1, ctx.shape[-1]))
-        c_kv, u_kv = ce.context_kv(ctx_bf), ue.context_kv(ctx_bf)
+        ctx_st = cast_as(st["act"], ctx.reshape(-1, ctx.shape[-1]))
+        c_kv, u_kv = ce.context_kv(ctx_st), ue.context_kv(ctx_st)
         memb = ce.map_embedding(x["image"]).repeat_interleave(st["n_cam"], dim=0).contiguous()  # 'b ... -> (b repeat) ...' (:842-843)
         if st["c_kv"] is None:
             st["c_kv"], st["u_kv"], st["map"] = c_kv, u_kv, memb

@@ -1,0 +1,324 @@
+"""The f16 instantiations of the denoising step's kernels (models with fp16 parameters): GEMM / implicit-GEMM convolution with
+every epilogue the step uses, fused attention, GroupNorm(+SiLU) and the glue, each against float64 (attention against fp32,
+within xformers' fp16 tolerance) and every output guard-banded as in test_kernel_edges_gpu.py."""
+import os
+
+import pytest
+import torch
+import torch.nn.functional as F
+
+pytestmark = pytest.mark.gpu
+
+from magicdrive_b200 import f16_ops, ops  # noqa: E402
+from magicdrive_b200.params import pack_geglu  # noqa: E402
+
+F16, F32, F64 = torch.float16, torch.float32, torch.float64
+G = 128  # guard rows before and after every output
+_FILL = {F16: (torch.int16, 0x7E5A), F32: (torch.int32, 0x7FA5A5A5)}  # NaN bit patterns no kernel produces
+
+
+class Guarded:
+    """A [rows, cols] output at column `col0` of a [G + rows + G, ld] NaN-filled buffer."""
+
+    def __init__(self, rows, cols, dtype=F16, ld=None, col0=0):
+        self.rows, self.cols, self.col0, self.ld = rows, cols, col0, ld or cols
+        self.itype, self.fill = _FILL[dtype]
+        self.buf = torch.empty((rows + 2 * G, self.ld), dtype=dtype, device="cuda")
+        self.buf.view(self.itype).fill_(self.fill)
+        self.out = self.buf[G:G + rows, col0:col0 + cols]
+
+    def check(self, what=""):
+        torch.cuda.synchronize()
+        bits = self.buf.view(self.itype)
+        outside = torch.ones_like(bits, dtype=torch.bool)
+        outside[G:G + self.rows, self.col0:self.col0 + self.cols] = False
+        assert not ((bits != self.fill) & outside).any(), f"{what}: guard elements overwritten"
+        assert not (self.out.view(self.itype) == self.fill).any(), f"{what}: output elements never written"
+
+
+def _gen(seed):
+    return torch.Generator(device="cuda").manual_seed(seed)
+
+
+def _randn(*shape, g, scale=1.0):
+    return (torch.randn(*shape, device="cuda", generator=g) * scale).to(F16)
+
+
+def _close_f16(out, ref, what=""):
+    """Every element within one f16 ulp of the float64 reference (plus 1e-4 of the largest |ref| for the fp32 accumulation
+    order and the subnormal range)."""
+    ref = ref.to(F64)
+    err = (out.to(F64) - ref).abs()
+    ulp = torch.exp2(torch.floor(torch.log2(ref.abs().clamp_min(2.0 ** -14))) - 10)
+    tol = ulp + 1e-4 * ref.abs().max()
+    bad = (err > tol).nonzero()
+    assert bad.shape[0] == 0, f"{what}: {bad.shape[0]} elements off, first at {tuple(bad[0].tolist())}, " \
+                              f"max err {err.max().item():.3e} (max |ref| {ref.abs().max().item():.3e})"
+
+
+def _conv_ref(a, w, n, h, wd, cin, cout, taps, pad):
+    x = a.to(F64).reshape(n, h, wd, cin).permute(0, 3, 1, 2)
+    k = w.to(F64).reshape(cout, taps, taps, cin).permute(0, 3, 1, 2)
+    return F.conv2d(x, k, padding=pad).permute(0, 2, 3, 1).reshape(-1, cout)
+
+
+# ---------------------------------------------------------------------------------------------------------------- GEMM
+@pytest.mark.parametrize("bn", [64, 128, 160, 256])
+@pytest.mark.parametrize("m,k,n", [(300, 320, 320), (1000, 136, 168), (129, 64, 512)])
+def test_linear_bias_residual_scale(cuda_lib, bn, m, k, n):
+    g = _gen(1)
+    a, w = _randn(m, k, g=g), _randn(n, k, g=g, scale=k ** -0.5)
+    bias, res = torch.randn(n, device="cuda", generator=g), _randn(m, n, g=g)
+    o = Guarded(m, n)
+    wk = F.pad(w, (0, -k % 64))  # K64 layout: a partial last K block reads zeros past k
+    ops.linear(a, wk, bias=bias, residual=res, out=o.out, ldo=n, out_scale=0.7, force_block_n=bn, allow_split_k=False)
+    o.check(f"linear bn={bn}")
+    _close_f16(o.out, 0.7 * (a.to(F64) @ w.to(F64).T + bias.to(F64)) + res.to(F64), f"linear bn={bn} {m}x{k}x{n}")
+
+
+@pytest.mark.parametrize("n_img,h,w,c0,c1,cout", [(2, 14, 25, 64, 0, 128), (3, 7, 13, 64, 128, 160), (1, 9, 11, 40, 24, 64)])
+def test_conv3x3_two_sources_rowbias(cuda_lib, n_img, h, w, c0, c1, cout):
+    """Implicit-GEMM 3x3 convolution over the concat of two f16 sources, with the per-image time shift."""
+    from magicdrive_b200.params import pack_conv_weight_k64
+    g = _gen(2)
+    pix = n_img * h * w
+    a0, a1 = _randn(pix, c0, g=g), _randn(pix, max(c1, 8), g=g)
+    wt = torch.randn(cout, c0 + c1, 3, 3, device="cuda", generator=g) * (9 * (c0 + c1)) ** -0.5
+    wk = pack_conv_weight_k64(wt.to(F16).float(), splits=[c0, c1] if c1 else None, dtype=F16)
+    bias, rowbias = torch.randn(cout, device="cuda", generator=g), torch.randn(n_img, cout, device="cuda", generator=g)
+    o = Guarded(pix, cout)
+    ops.gemm_conv(a0, wk, n_img=n_img, h_in=h, w_in=w, c0=c0, lda0=c0, a1=a1 if c1 else None, c1=c1, lda1=a1.stride(0),
+                  n_out=cout, taps=3, pad=1, bias=bias, rowbias=rowbias, out=o.out, ldo=cout)
+    o.check("conv3x3")
+    x = torch.cat([a0.to(F64), a1[:, :c1].to(F64)], 1) if c1 else a0.to(F64)
+    ref = _conv_ref(x, wt.to(F16).permute(0, 2, 3, 1).reshape(cout, -1), n_img, h, w, c0 + c1, cout, 3, 1)
+    ref = ref + bias.to(F64) + rowbias.to(F64).repeat_interleave(h * w, 0)
+    _close_f16(o.out, ref, "conv3x3 two sources")
+
+
+def test_forced_split_k_with_residual_and_f32_output(cuda_lib):
+    g = _gen(3)
+    m, k, n = 200, 1280, 320
+    a, w = _randn(m, k, g=g), _randn(n, k, g=g, scale=k ** -0.5)
+    bias, res = torch.randn(n, device="cuda", generator=g), _randn(m, n, g=g)
+    ref = a.to(F64) @ w.to(F64).T + bias.to(F64)
+    o = Guarded(m, n)
+    ops.linear(a, w, bias=bias, residual=res, out=o.out, ldo=n, force_splits=4)
+    o.check("split-K")
+    _close_f16(o.out, ref + res.to(F64), "split-K + residual")
+    o32 = Guarded(m, n, F32)
+    ops.linear(a, w, bias=bias, out=o32.out, ldo=n, out_f32=True, force_splits=3)
+    o32.check("split-K fp32")
+    err = (o32.out.to(F64) - ref).abs().max().item()
+    assert err <= 3e-5 * ref.abs().max().item(), err
+
+
+@pytest.mark.parametrize("bn", [128, 160, 256])
+def test_residual_aliases_the_output(cuda_lib, bn):
+    """The zero convolutions add into the UNet skip in place: residual == out, in a column slice of a wider buffer."""
+    g = _gen(4)
+    m, k, n, ld = 700, 320, 320, 640
+    a, w = _randn(m, k, g=g), _randn(n, k, g=g, scale=k ** -0.5)
+    buf = _randn(m, ld, g=g)
+    before = buf.clone()
+    view = buf[:, 160:160 + n]
+    ops.linear(a, w, residual=view, out=view, ldo=ld, out_scale=0.5, force_block_n=bn, allow_split_k=False)
+    torch.cuda.synchronize()
+    _close_f16(view, 0.5 * (a.to(F64) @ w.to(F64).T) + before[:, 160:160 + n].to(F64), f"in place bn={bn}")
+    assert torch.equal(buf[:, :160], before[:, :160]) and torch.equal(buf[:, 160 + n:], before[:, 160 + n:])
+
+
+def test_geglu(cuda_lib):
+    g = _gen(5)
+    m, k, inner = 333, 320, 1280
+    a = _randn(m, k, g=g)
+    wf, bf = torch.randn(2 * inner, k, device="cuda", generator=g) * k ** -0.5, torch.randn(2 * inner, device="cuda", generator=g)
+    wp, bp = pack_geglu(wf, bf, dtype=F16)
+    o = Guarded(m, inner)
+    ops.linear(a, wp, bias=bp, geglu=True, out=o.out, ldo=inner)
+    o.check("geglu")
+    y = a.to(F64) @ wf.to(F16).to(F64).T + bf.to(F64)
+    _close_f16(o.out, y[:, :inner] * F.gelu(y[:, inner:]), "geglu")
+
+
+@pytest.mark.parametrize("offset", [0.0, 30.0])
+def test_row_statistics_and_folded_layernorm(cuda_lib, offset):
+    """The producer's row statistics are those of its f16-rounded stored values; the consumer folds LayerNorm(gamma, beta)
+    into its weights (W * gamma rounded to f16) and normalises with them."""
+    g = _gen(6)
+    m, k, c, n = 500, 320, 320, 960
+    a, w = _randn(m, k, g=g), _randn(c, k, g=g, scale=k ** -0.5)
+    bias = torch.randn(c, device="cuda", generator=g) + offset
+    x, st = ops.linear(a, w, bias=bias, emit_stats=True)
+    torch.cuda.synchronize()
+    xs = x.to(F64)
+    tot = st.data.to(F64).sum(1)
+    assert torch.allclose(tot[:, 0], xs.sum(1), rtol=1e-5, atol=1e-4 * c), "row sums"
+    assert torch.allclose(tot[:, 1], (xs * xs).sum(1), rtol=1e-5, atol=1e-4 * c), "row sums of squares"
+    gam, beta = 1 + 0.1 * torch.randn(c, device="cuda", generator=g), 0.1 * torch.randn(c, device="cuda", generator=g)
+    wl, bl = torch.randn(n, c, device="cuda", generator=g) * c ** -0.5, torch.randn(n, device="cuda", generator=g)
+    wg = (wl * gam[None]).to(F16)
+    cvec = wl @ beta + bl
+    o = Guarded(m, n)
+    ops.linear(x, wg, bias=cvec, ln=st, ln_colsum=wg.float().sum(1), ln_eps=1e-5, out=o.out, ldo=n)
+    o.check("folded layernorm")
+    ref = F.layer_norm(xs, (c,), eps=1e-5) @ wg.to(F64).T + cvec.to(F64)
+    err = (o.out.to(F64) - ref).abs()
+    assert (err <= ref.abs() * 2.0 ** -10 + 2e-3 * ref.abs().max()).all(), err.max().item()
+
+
+def test_f16_rejections(cuda_lib):
+    g = _gen(7)
+    a, w = _randn(128, 64, g=g), _randn(64, 64, g=g)
+    for kw in (dict(quick_gelu=True), dict(relu=True), dict(kernel_variant=3)):
+        with pytest.raises(Exception):
+            ops.linear(a, w, **kw)
+
+
+# ---------------------------------------------------------------------------------------------------------- attention
+def _attn_ref(q, k, v, b, bkv, heads, lq, lk, d, scale, n_keys=None):
+    qh = q.float().reshape(b, lq, heads, d).transpose(1, 2)
+    kh = k.float().reshape(bkv, lk, heads, d).transpose(1, 2)
+    vh = v.float().reshape(bkv, lk, heads, d).transpose(1, 2)
+    s = qh @ kh.transpose(-1, -2) * scale
+    if n_keys is not None:
+        s = s.masked_fill(torch.arange(lk, device="cuda")[None, None, None] >= n_keys[:, None, None, None], float("-inf"))
+    return (torch.softmax(s, -1) @ vh).transpose(1, 2).reshape(b * lq, heads * d)
+
+
+def _xformers_close(out, ref, what=""):
+    assert torch.allclose(out.float(), ref, atol=4e-3, rtol=4e-4), f"{what}: max err {(out.float() - ref).abs().max().item():.3e}"
+
+
+@pytest.mark.parametrize("d", [32, 40, 64, 80, 160])
+@pytest.mark.parametrize("lq,lk", [(350, 350), (700, 97)])
+def test_attention(cuda_lib, d, lq, lk):
+    g = _gen(8)
+    b, heads = 3, 2
+    q, k, v = (_randn(n, heads * d, g=g) for n in (b * lq, b * lk, b * lk))
+    o = Guarded(b * lq, heads * d)
+    ops.attention(q, k, v, b=b, heads=heads, lq=lq, lk=lk, d=d, ldq=heads * d, ldk=heads * d, ldv=heads * d,
+                  scale=d ** -0.5, out=o.out)
+    o.check(f"attention d={d}")
+    _xformers_close(o.out, _attn_ref(q, k, v, b, b, heads, lq, lk, d, d ** -0.5), f"attention d={d}")
+
+
+@pytest.mark.parametrize("d", [40, 64, 80])
+def test_attention_add_sets_with_empty_slots(cuda_lib, d):
+    """Cross-view "add" mode: per-set softmax, each set's output rounded to f16 before the sum in slot order; -1 slots add
+    nothing, [a, -1, b] is bitwise [a, b] and a row with no present set is zero."""
+    g = _gen(9)
+    b, heads, L = 4, 2, 200
+    qkv = _randn(b * L, 3 * heads * d, g=g)
+    C = heads * d
+    q, k, v = qkv, qkv[:, C:], qkv[:, 2 * C:]
+    idx3 = torch.tensor([[1, -1, 3], [0, -1, 2], [-1, -1, -1], [2, -1, 0]], dtype=torch.int32, device="cuda")
+    idx2 = torch.tensor([[1, 3], [0, 2], [-1, -1], [2, 0]], dtype=torch.int32, device="cuda")
+    kw = dict(b=b, heads=heads, lq=L, lk=L, d=d, ldq=3 * C, ldk=3 * C, ldv=3 * C, scale=d ** -0.5)
+    o3 = ops.attention(q, k, v, kv_index=idx3, n_sets=3, **kw)
+    o2 = ops.attention(q, k, v, kv_index=idx2, n_sets=2, **kw)
+    torch.cuda.synchronize()
+    assert torch.equal(o3, o2)
+    for i, row in enumerate(idx2.tolist()):
+        present = [j for j in row if j >= 0]
+        if not present:
+            assert (o3.reshape(b, L, C)[i] == 0).all()
+            continue
+        t = qkv.reshape(b, L, 3 * C)
+        qi = t[i, :, :C].contiguous()
+        ref = torch.zeros(L, C, device="cuda")
+        for j in present:
+            kj, vj = t[j, :, C:2 * C].contiguous(), t[j, :, 2 * C:].contiguous()
+            ref = ref + _attn_ref(qi, kj, vj, 1, 1, heads, L, L, d, d ** -0.5).half().float()
+        _xformers_close(o3.reshape(b, L, C)[i], ref, f"add mode d={d} row {i}")
+
+
+@pytest.mark.parametrize("d", [40, 80, 160])
+def test_attention_kv_len_resident_and_multi_q_bitwise(cuda_lib, d):
+    """kv_len (the KVRES kernel of a box capacity) is bitwise the exact-length launch; multi-Q launches are bitwise the
+    one-query-tile-per-CTA launch."""
+    g = _gen(10)
+    b, heads, lq, cap = 12, 8, 1400, 256
+    C = heads * d
+    q, kv = _randn(b * lq, C, g=g), _randn(b * cap, 2 * C, g=g)
+    lens = torch.tensor([78 + (7 * i) % 150 for i in range(b)], dtype=torch.int32, device="cuda")
+    kw = dict(b=b, heads=heads, lq=lq, d=d, ldq=C, ldk=2 * C, ldv=2 * C, scale=d ** -0.5)
+    o = ops.attention(q, kv, kv[:, C:], lk=cap, kv_len=lens, **kw)
+    torch.cuda.synchronize()
+    for i in (0, 5, 11):
+        n = int(lens[i])
+        kvi = kv.reshape(b, cap, 2 * C)[i, :n].contiguous()
+        oi = ops.attention(q.reshape(b, lq, C)[i].contiguous(), kvi, kvi[:, C:], lk=n, **dict(kw, b=1))
+        torch.cuda.synchronize()
+        assert torch.equal(o.reshape(b, lq, C)[i], oi), (d, i)
+    ref = _attn_ref(q, kv[:, :C].contiguous(), kv[:, C:].contiguous(), b, b, heads, lq, cap, d, d ** -0.5, lens.long())
+    _xformers_close(o, ref, f"kv_len d={d}")
+    # multi-Q: one key tile (lk <= BN), more query tiles than SMs hold at once
+    lk = 64
+    kv2 = kv[: b * lk]
+    prev = os.environ.get("MDB_ATTN_MULTIQ")
+    try:
+        os.environ["MDB_ATTN_MULTIQ"] = "0"
+        one = ops.attention(q, kv2, kv2[:, C:], lk=lk, **kw)
+        os.environ.pop("MDB_ATTN_MULTIQ")
+        multi = ops.attention(q, kv2, kv2[:, C:], lk=lk, **kw)
+        torch.cuda.synchronize()
+    finally:
+        if prev is not None:
+            os.environ["MDB_ATTN_MULTIQ"] = prev
+    assert torch.equal(one, multi), d
+
+
+# ---------------------------------------------------------------------------------------------------------- GroupNorm
+@pytest.mark.parametrize("rows", ["0", "1"])
+@pytest.mark.parametrize("n_img,hw,c0,c1,silu", [(12, 350, 320, 0, True), (6, 1400, 640, 320, True), (4, 91, 1280, 0, False)])
+def test_groupnorm(cuda_lib, monkeypatch, rows, n_img, hw, c0, c1, silu):
+    """gn_fused_kernel (MDB_GN_ROWS=0) and the cluster gn_rows_kernel (=1), two sources included."""
+    monkeypatch.setenv("MDB_GN_ROWS", rows)
+    g = _gen(11)
+    x0, x1 = _randn(n_img * hw, c0, g=g, scale=3.0), _randn(n_img * hw, max(c1, 8), g=g)
+    x0 = (x0.float() + 5.0).half()
+    gam, beta = 1 + 0.1 * torch.randn(c0 + c1, device="cuda", generator=g), 0.1 * torch.randn(c0 + c1, device="cuda", generator=g)
+    out = ops.groupnorm(x0, c0, c0, n_img, hw, gam, beta, 1e-5, silu, x1=x1 if c1 else None, c1=c1, ld1=x1.stride(0))
+    torch.cuda.synchronize()
+    assert out.dtype == F16
+    x = torch.cat([x0.to(F64), x1[:, :c1].to(F64)], 1) if c1 else x0.to(F64)
+    y = F.group_norm(x.reshape(n_img, hw, -1).permute(0, 2, 1), 32, gam.to(F64), beta.to(F64), 1e-5)
+    y = (F.silu(y) if silu else y).permute(0, 2, 1).reshape(n_img * hw, -1)
+    _close_f16(out, y, f"groupnorm rows={rows}")
+
+
+# ---------------------------------------------------------------------------------------------------------------- glue
+def test_conversions_over_every_f16_pattern(cuda_lib):
+    bits = torch.arange(-32768, 32768, dtype=torch.int32, device="cuda").to(torch.int16)
+    h = bits.view(F16)
+    f = f16_ops.f16_to_f32(h.contiguous())
+    torch.cuda.synchronize()
+    assert torch.equal(f.view(torch.int32), h.float().view(torch.int32))
+    # every finite pattern, and the midpoints between neighbours (ties round to even) and just off them
+    fin = f[torch.isfinite(f)].to(F64).unique()
+    mids = (fin[1:] + fin[:-1]) / 2
+    x = torch.cat([fin, mids, mids * (1 + 2.0 ** -20), mids * (1 - 2.0 ** -20), torch.tensor([7e4, -7e4, 65520.0], device="cuda",
+                                                                                             dtype=F64)]).float()
+    x = torch.cat([x, torch.tensor([float("nan"), float("inf"), -float("inf")], device="cuda")])
+    y = f16_ops.f32_to_f16(x.contiguous())
+    torch.cuda.synchronize()
+    ref = x.half()
+    same = (y.view(torch.int16) == ref.view(torch.int16)) | (torch.isnan(y) & torch.isnan(ref))
+    assert same.all(), x[~same][:8]
+
+
+def test_add_upsample_pack_bitwise(cuda_lib):
+    g = _gen(12)
+    a, b = _randn(6 * 28 * 50, 320, g=g, scale=40.0), _randn(6 * 28 * 50, 320, g=g, scale=40.0)
+    s = ops.add(a, b)
+    x = _randn(2 * 14 * 25, 640, g=g)
+    u = ops.upsample_nearest(x, 2, 14, 25, 640, 28, 50)
+    lat = torch.randn(6 * 28 * 50, 4, device="cuda", generator=g)
+    p = f16_ops.pack_latents_f16(lat, 64, repeat=2)
+    torch.cuda.synchronize()
+    assert s.dtype == u.dtype == p.dtype == F16
+    assert torch.equal(s, a + b)
+    ref = F.interpolate(x.reshape(2, 14, 25, 640).permute(0, 3, 1, 2), size=(28, 50), mode="nearest")
+    assert torch.equal(u, ref.permute(0, 2, 3, 1).reshape(-1, 640))
+    assert torch.equal(p, F.pad(lat, (0, 60)).half().repeat(2, 1))
