@@ -38,6 +38,8 @@ def f16_to_f32(x):
 def pack_latents_f16(x, cpad: int = 64, repeat: int = 1):
     """[pix, cin] fp32/f16 -> f16 [repeat*pix, cpad] zero-padded channels (the conv_in operand of an fp16 model)."""
     _need_cuda(x)
+    if x.dtype not in (F32, F16):  # the kernel reads any other source as f16 bits
+        raise TypeError(f"pack_latents_f16: x is {x.dtype}, expected float32 or float16")
     pix, cin = x.shape
     out = torch.empty((repeat * pix, cpad), dtype=F16, device=x.device)
     check(_lib.lib().mdb_pack_latents_f16(_ptr(x), int(x.dtype == F32), pix, cin, cpad, repeat, _ptr(out), _stream()),

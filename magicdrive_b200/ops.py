@@ -4,7 +4,8 @@ torch is plumbing only: it owns device memory and the CUDA stream; every functio
 `libmagicdrive_b200.so` and raises if the library / a CUDA device is unavailable (no CPU or eager fallback).
 Feature maps are NHWC bf16 ("channels innermost") everywhere; a token matrix [tokens, C] is the same layout.  The operators of
 the denoising step (gemm_conv, groupnorm, attention, add, upsample_nearest, linear_small's weights) also take f16 tensors --
-the engines of models with fp16 parameters -- and then run their f16 kernels: the element type follows the tensors passed in.
+the engines of models with fp16 parameters -- and then run their f16 kernels: the element type follows the tensors passed in,
+and an operand of the other type is a TypeError before anything is launched.
 The operators that only fp16 models need (fp32 <-> f16 conversion, f16 latent packing) are in f16_ops.py.
 
 One process drives ONE device (the launch contract: one process per GPU): the module-level workspace slot / launch counter and the
@@ -82,6 +83,21 @@ def _need_cuda(*ts):
             raise _lib.MdbError("magicdrive_b200 operators need CUDA tensors; there is no CPU fallback")
 
 
+def _need_dtype(op: str, dtype, **tensors):
+    """Raise TypeError unless every given tensor (None = absent) has `dtype`: a kernel reads raw bits in one element type, so
+    an operand of another type would be read as garbage rather than converted."""
+    for name, t in tensors.items():
+        if t is not None and t.dtype != dtype:
+            raise TypeError(f"{op}: {name} is {t.dtype}, expected {dtype}")
+
+
+def _act_dtype(op: str, t):
+    """The element type of an operator that runs bf16 or f16 kernels, taken from its first tensor."""
+    if t.dtype not in (BF16, F16):
+        raise TypeError(f"{op}: expected bfloat16 or float16 tensors, got {t.dtype}")
+    return t.dtype
+
+
 _ws = {}
 _ws_slot = 0
 
@@ -146,10 +162,9 @@ def gemm_conv(a0: torch.Tensor, w: torch.Tensor, *, n_img: int, h_in: int, w_in:
     output rows -> (out, RowStats).  quick_gelu: out = y * sigmoid(1.702 y) (CLIP's MLP activation)."""
     global _launches
     _need_cuda(a0, w)
-    act = F16 if a0.dtype == F16 else BF16  # mdb_gemm_desc.operand_dtype: a0, a1, w and residual share it
-    if act == F16:
-        assert w.dtype == F16 and (a1 is None or a1.dtype == F16) and (residual is None or residual.dtype == F16), \
-            "an f16 gemm_conv takes f16 weights, second source and residual"
+    act = _act_dtype("gemm_conv", a0)  # mdb_gemm_desc.operand_dtype: a0, a1, w, residual and a non-fp32 out share it
+    _need_dtype("gemm_conv", act, w=w, a1=a1, residual=residual)
+    _need_dtype("gemm_conv", F32 if out_f32 else act, out=out)
     th = taps if taps_h is None else taps_h
     tw = taps if taps_w is None else taps_w
     ph = pad if pad_h is None else pad_h
@@ -250,6 +265,7 @@ def conv_direct(x, wgt, bias, *, n, h, w, cin, cout, k, stride=(1, 1), pad=(1, 1
 def groupnorm(x0, c0, ld0, n_img, hw, gamma, beta, eps, silu, x1=None, c1=0, ld1=0, groups=32):
     global _launches
     _need_cuda(x0)
+    _need_dtype("groupnorm", _act_dtype("groupnorm", x0), x1=x1)
     f16 = x0.dtype == F16  # mdb_groupnorm_f16: f16 sources and output
     out = torch.empty((n_img * hw, c0 + c1), dtype=F16 if f16 else BF16, device=x0.device)
     stats = torch.empty((max(n_img, 160) * groups * 2,), dtype=F32, device=x0.device)  # scratch: per-(image | CTA run) group partials
@@ -293,6 +309,7 @@ def attention(q, k, v, *, b, heads, lq, lk, d, ldq, ldk, ldv, scale, kv_index=No
     b_kv = b if b_kv is None else b_kv
     global _launches
     _need_cuda(q, k, v)
+    _need_dtype("attention", _act_dtype("attention", q), k=k, v=v, out=out)
     if out is None:
         out = torch.empty((b * lq, heads * d), dtype=BF16, device=q.device)
     e0 = _prof_begin()
@@ -310,8 +327,12 @@ def attention_multi(q, sources, *, b, heads, lq, lk, d, ldq, scale, kv_index, n_
     kv_len: int32 [b] keys per query batch (mdb_attention_varlen), None = lk."""
     global _launches
     _need_cuda(q, *[t for s_ in sources for t in s_[:2]], kv_len)
+    act = _act_dtype("attention", q)
+    for i, s_ in enumerate(sources):
+        _need_dtype("attention", act, **{f"k of source {i}": s_[0], f"v of source {i}": s_[1]})
+    _need_dtype("attention", act, out=out)
     n = len(sources)
-    f16 = q.dtype == F16  # mdb_attention_varlen_f16 (kv_len may be None there)
+    f16 = act == F16  # mdb_attention_varlen_f16 (kv_len may be None there)
     if out is None:
         out = torch.empty((b * lq, heads * d), dtype=F16 if f16 else BF16, device=q.device)
     ks = (C.c_void_p * n)(*[s_[0].data_ptr() for s_ in sources])
@@ -383,6 +404,7 @@ def peer_barrier(flag_ptrs_dev: int, rank: int, world: int, channel: int, n_chan
 def add(a, b):
     global _launches
     _need_cuda(a, b)
+    _need_dtype("add", _act_dtype("add", a), b=b)
     out = torch.empty_like(a)
     fn = _lib.lib().mdb_add_f16 if a.dtype == F16 else _lib.lib().mdb_add  # f16 a and b: mdb_add_f16
     check(fn(_ptr(a), _ptr(b), _ptr(out), a.numel(), _stream()), "mdb_add")
@@ -460,6 +482,8 @@ def linear_small(x, w, bias=None, pre_silu=False, post_silu=False):
     """x fp32 [m, k]; w bf16 (or f16: mdb_linear_small_f16) [n, k]; returns fp32 [m, n]."""
     global _launches
     _need_cuda(x, w)
+    _need_dtype("linear_small", F32, x=x)
+    _act_dtype("linear_small", w)
     m, k = x.shape
     n = w.shape[0]
     out = torch.empty((m, n), dtype=F32, device=x.device)

@@ -2,10 +2,15 @@
 images per tile, split-K finalisation, strided inputs and outputs, multi-source attention, long sequences, every GroupNorm
 kernel, the direct convolution and the adaptive pool.
 
-Every reference is computed in float64 on the GPU from the same bf16-rounded inputs.  Every output is written into a larger
-buffer pre-filled with a NaN bit pattern: at least one full 128-row M tile of guard rows before and after the output, and
-guard columns on both sides whenever the row stride exceeds the written width.  After each call every guard element must be
-bitwise unchanged and no interior element may still hold the fill pattern."""
+The GEMM, attention and GroupNorm kernels have f16 twins (the denoising step of a model with fp16 parameters) that share
+their bodies through Act<F16> (csrc/ptx.cuh); those tests take the element type `dt` (bf16 | f16, `with_dt`) and run both at
+the same edges, the f16 cases under ids that start with "f16-".  The VAE launches, the direct convolution and the adaptive
+pool are bf16 / fp32 only.
+
+Every reference is computed in float64 on the GPU from the same bf16- (or f16-) rounded inputs.  Every output is written
+into a larger buffer pre-filled with a NaN bit pattern: at least one full 128-row M tile of guard rows before and after the
+output, and guard columns on both sides whenever the row stride exceeds the written width.  After each call every guard
+element must be bitwise unchanged and no interior element may still hold the fill pattern."""
 import math
 
 import pytest
@@ -16,12 +21,22 @@ pytestmark = pytest.mark.gpu
 
 from magicdrive_b200 import ops  # noqa: E402
 
-BF16, F32, F64 = torch.bfloat16, torch.float32, torch.float64
+BF16, F16, F32, F64 = torch.bfloat16, torch.float16, torch.float32, torch.float64
 G = 128  # guard rows before and after every output: one full GEMM M tile
-_FILL = {BF16: (torch.int16, 0x7FA5), F32: (torch.int32, 0x7FA5A5A5)}  # NaN bit patterns no kernel produces
+_FILL = {BF16: (torch.int16, 0x7FA5), F16: (torch.int16, 0x7E5A), F32: (torch.int32, 0x7FA5A5A5)}  # NaNs no kernel produces
 
 
 # ---------------------------------------------------------------------------------------------------------- helpers
+def with_dt(values, ids=None, f16=None):
+    """pytest params (dt, *value) for the element types of the kernels with f16 twins: every value in bf16 under the id it
+    has without `dt` (so the bf16 cases keep the ids they had before the f16 twins existed), then in f16 under "f16-" + that
+    id, for every value or only those whose id is in `f16`."""
+    values = [v if isinstance(v, tuple) else (v,) for v in values]
+    ids = ids or ["-".join(str(x) for x in v) for v in values]
+    return ([pytest.param(BF16, *v, id=i) for v, i in zip(values, ids)] +
+            [pytest.param(F16, *v, id=f"f16-{i}") for v, i in zip(values, ids) if f16 is None or i in f16])
+
+
 def _gen(seed):
     return torch.Generator(device="cuda").manual_seed(seed)
 
@@ -67,6 +82,19 @@ def _close_bf16(out, ref, what=""):
                               f"max err {err.max().item():.3e} (max |ref| {ref.abs().max().item():.3e})"
 
 
+def _close_f16(out, ref, what=""):
+    """Every element within one f16 ulp of the float64 reference (the ulp floored at 2^-24 in the subnormal range), plus 1e-4
+    of the largest |ref| for the fp32 accumulation order.  Every f16 store rounds an fp32 value to nearest even (Act<true> in
+    csrc/ptx.cuh), so a store at any coarser precision (bf16's 8 bits) fails it."""
+    ref = ref.to(F64)
+    err = (out.to(F64) - ref).abs()
+    ulp = torch.exp2(torch.floor(torch.log2(ref.abs().clamp_min(2.0 ** -14))) - 10)
+    tol = ulp + 1e-4 * ref.abs().max()
+    bad = (err > tol).nonzero()
+    assert bad.shape[0] == 0, f"{what}: {bad.shape[0]} elements off, first at {tuple(bad[0].tolist())}, " \
+                              f"max err {err.max().item():.3e} (max |ref| {ref.abs().max().item():.3e})"
+
+
 def _close_f32(out, ref, what=""):
     ref = ref.to(F64)
     err = (out.to(F64) - ref).abs()
@@ -77,7 +105,7 @@ def _close_f32(out, ref, what=""):
 
 
 def _close(out, ref, what=""):
-    (_close_f32 if out.dtype == F32 else _close_bf16)(out, ref, what)
+    {F32: _close_f32, BF16: _close_bf16, F16: _close_f16}[out.dtype](out, ref, what)
 
 
 def _conv_ref(srcs, n, h, w, wmat, taps, stride=1, pad=0):
@@ -105,26 +133,26 @@ VARIANT_IDS = ["planner", "nosplit"]
 
 
 def _run_conv(*, n, h, w, c0, co, taps=1, stride=1, pad=0, lda0=None, c1=0, bias=True, rowbias=None, residual=False,
-              out_f32=False, out_scale=1.0, ldo=None, col0=0, variant=0, seed=0, a0=None, **kw):
-    """One guarded gemm_conv launch on random bf16 operands, checked against float64; returns (Guarded, ref)."""
+              out_f32=False, out_scale=1.0, ldo=None, col0=0, variant=0, seed=0, a0=None, dt=BF16, **kw):
+    """One guarded gemm_conv launch on random `dt` (bf16 | f16) operands, checked against float64; returns (Guarded, ref)."""
     g = _gen(seed)
     ho = (h + 2 * pad - taps) // stride + 1
     wo = (w + 2 * pad - taps) // stride + 1
     pix_in, pix = n * h * w, n * ho * wo
     lda0 = lda0 or c0
     if a0 is None:
-        a0 = _bf(_randn(pix_in, lda0, g=g))[:, :c0]
-    a1 = _bf(_randn(pix_in, c1, g=g)) if c1 else None
+        a0 = _randn(pix_in, lda0, g=g).to(dt)[:, :c0]
+    a1 = _randn(pix_in, c1, g=g).to(dt) if c1 else None
     k = taps * taps * (c0 + c1)
-    wm = _bf(_randn(co, k, g=g, scale=1 / math.sqrt(k)))
+    wm = _randn(co, k, g=g, scale=1 / math.sqrt(k)).to(dt)
     b = _randn(co, g=g) if bias else None
     rb = None
     if rowbias == "image":  # per-image shift, a column slice of a wider table (temb_all[:, off:off + cout])
         rb = _randn(n, co + 72, g=g)[:, 40:40 + co]
     elif rowbias == "shared":  # one row for every image
         rb = _randn(1, co, g=g)
-    res = _bf(_randn(pix, co, g=g)) if residual else None
-    out = Guarded(pix, co, F32 if out_f32 else BF16, ld=ldo, col0=col0)
+    res = _randn(pix, co, g=g).to(dt) if residual else None
+    out = Guarded(pix, co, F32 if out_f32 else dt, ld=ldo, col0=col0)
     ops.gemm_conv(a0, wm, n_img=n, h_in=h, w_in=w, c0=c0, lda0=lda0, a1=a1, c1=c1, lda1=c1, n_out=co, taps=taps,
                   stride=stride, pad=pad, bias=b, rowbias=rb, residual=res, ldr=co, out=out.out, ldo=out.ld,
                   out_f32=out_f32, out_scale=out_scale, kernel_variant=variant, **kw)
@@ -155,13 +183,16 @@ PRODUCT_CONVS = {
     "vae_shortcut_224x400": (1, 224, 400, 256, 128, 1, 1, 0, {}),
     "downsample_s2": (12, 28, 50, 320, 320, 3, 2, 1, {}),
 }
+# the UNet / ControlNet launches in both element types; the VAE decoder is bf16 whatever its parameters (INTEGRATION.md)
+PRODUCT_F16 = ("conv_in", "conv_out", "downsample_s2")
 
 
 @pytest.mark.parametrize("variant", VARIANTS, ids=VARIANT_IDS)
-@pytest.mark.parametrize("case", list(PRODUCT_CONVS))
-def test_gemm_product_convs(cuda_lib, case, variant):
+@pytest.mark.parametrize("dt,case", with_dt(list(PRODUCT_CONVS), f16=PRODUCT_F16))
+def test_gemm_product_convs(cuda_lib, dt, case, variant):
     n, h, w, c0, co, taps, stride, pad, extra = PRODUCT_CONVS[case]
-    out, ref = _run_conv(n=n, h=h, w=w, c0=c0, co=co, taps=taps, stride=stride, pad=pad, variant=variant, seed=1, **extra)
+    out, ref = _run_conv(n=n, h=h, w=w, c0=c0, co=co, taps=taps, stride=stride, pad=pad, variant=variant, seed=1, dt=dt,
+                         **extra)
     out.check(case)
     _close(out.out, ref, case)
 
@@ -205,37 +236,37 @@ M_TAILS = [
 
 
 @pytest.mark.parametrize("variant", VARIANTS, ids=VARIANT_IDS)
-@pytest.mark.parametrize("n,h,w,taps,stride", M_TAILS)
-def test_gemm_m_tails(cuda_lib, n, h, w, taps, stride, variant):
+@pytest.mark.parametrize("dt,n,h,w,taps,stride", with_dt(M_TAILS))
+def test_gemm_m_tails(cuda_lib, dt, n, h, w, taps, stride, variant):
     pad = taps // 2
     out, ref = _run_conv(n=n, h=h, w=w, c0=128, co=192, taps=taps, stride=stride, pad=pad, rowbias="image",
-                         residual=True, variant=variant, seed=3)
+                         residual=True, variant=variant, seed=3, dt=dt)
     out.check()
-    _close_bf16(out.out, ref)
+    _close(out.out, ref)
 
 
 @pytest.mark.parametrize("variant", VARIANTS, ids=VARIANT_IDS)
 @pytest.mark.parametrize("stats", [False, True], ids=["plain", "stats"])
 @pytest.mark.parametrize("bn", [64, 128, 160, 256])
-@pytest.mark.parametrize("n_out", [8, 40, 136, 264, 520])  # a tail past every block width
-def test_gemm_n_tails(cuda_lib, n_out, bn, stats, variant):
+@pytest.mark.parametrize("dt,n_out", with_dt([8, 40, 136, 264, 520]))  # a tail past every block width
+def test_gemm_n_tails(cuda_lib, dt, n_out, bn, stats, variant):
     g = _gen(4)
     m, k = 1000, 320
-    x = _bf(_randn(m, k, g=g))
-    w = _bf(_randn(n_out, k, g=g, scale=1 / math.sqrt(k)))
+    x = _randn(m, k, g=g).to(dt)
+    w = _randn(n_out, k, g=g, scale=1 / math.sqrt(k)).to(dt)
     b = _randn(n_out, g=g)
-    r = _bf(_randn(m, n_out, g=g))
-    out = Guarded(m, n_out)
+    r = _randn(m, n_out, g=g).to(dt)
+    out = Guarded(m, n_out, dt)
     res = ops.linear(x, w, bias=b, residual=r, out=out.out, ldo=n_out, force_block_n=bn, kernel_variant=variant,
                      emit_stats=stats)
     out.check()
     ref = x.to(F64) @ w.to(F64).t() + b.to(F64) + r.to(F64)
-    _close_bf16(out.out, ref)
+    _close(out.out, ref)
     if stats:
         st = res[1]
         assert st.parts == (n_out + bn - 1) // bn and st.data.shape == (m, st.parts, 2)
         s = st.data.to(F64).sum(1)
-        # the statistics are taken from the values as stored, after their rounding to bf16
+        # the statistics are taken from the values as stored, after their rounding to bf16 / f16
         stored = out.out.to(F64)
         torch.testing.assert_close(s[:, 0], stored.sum(1), rtol=0, atol=2e-3)
         torch.testing.assert_close(s[:, 1], (stored ** 2).sum(1), rtol=1e-5, atol=2e-3)
@@ -243,37 +274,39 @@ def test_gemm_n_tails(cuda_lib, n_out, bn, stats, variant):
 
 @pytest.mark.parametrize("variant", VARIANTS, ids=VARIANT_IDS)
 @pytest.mark.parametrize("rowbias", ["image", "shared"])
-@pytest.mark.parametrize("splits", [2, 3, 7])
-def test_gemm_split_k_epilogue(cuda_lib, splits, rowbias, variant):
-    """Split-K finalisation with the UNet resnet's epilogue: bf16 output + bias + time-embedding shift (per image, or one
-    row for all) + scale + residual; the result is bitwise reproducible."""
+@pytest.mark.parametrize("dt,splits", with_dt([2, 3, 7]))
+def test_gemm_split_k_epilogue(cuda_lib, dt, splits, rowbias, variant):
+    """Split-K finalisation with the UNet resnet's epilogue: bf16 / f16 output + bias + time-embedding shift (per image, or
+    one row for all) + scale + residual; the result is bitwise reproducible."""
     kw = dict(n=3, h=14, w=25, c0=640, co=640, taps=3, pad=1, rowbias=rowbias, residual=True, out_scale=0.75,
-              force_splits=splits, variant=variant, seed=5)
+              force_splits=splits, variant=variant, seed=5, dt=dt)
     out, ref = _run_conv(**kw)
     out.check()
-    _close_bf16(out.out, ref)
+    _close(out.out, ref)
     again, _ = _run_conv(**kw)
     assert torch.equal(out.out.view(torch.int16), again.out.view(torch.int16))
 
 
 @pytest.mark.parametrize("variant", VARIANTS, ids=VARIANT_IDS)
-@pytest.mark.parametrize("taps,stride", [(3, 1), (1, 1), (3, 2)])
-def test_gemm_strided_sources_and_output(cuda_lib, taps, stride, variant):
+@pytest.mark.parametrize("dt,taps,stride", with_dt([(3, 1), (1, 1), (3, 2)]))
+def test_gemm_strided_sources_and_output(cuda_lib, dt, taps, stride, variant):
     """Source 0 a channel slice of a wider buffer (lda0 > c0), a second concatenated source, output into a column slice."""
     out, ref = _run_conv(n=3, h=14, w=25, c0=320, lda0=448, c1=192, co=320, taps=taps, stride=stride, pad=taps // 2,
-                         residual=True, ldo=512, col0=128, variant=variant, seed=6)
+                         residual=True, ldo=512, col0=128, variant=variant, seed=6, dt=dt)
     out.check()
-    _close_bf16(out.out, ref)
+    _close(out.out, ref)
 
 
 # ------------------------------------------------------------------------------------------------------ attention
 ATTN_KERNELS = ["tc2", "tc2d", "tc"]  # key-tile width: per head dim (default) | 64 keys | 128 keys
+# MDB_ATTN_KERNEL is a bf16 A/B switch: the f16 kernels have the default key-tile width only (capi_attention.cu)
+ATTN_DT_KERNELS = with_dt(ATTN_KERNELS, f16=("tc2",))
 HEADS = {32: 2, 40: 8, 64: 2, 80: 4, 160: 2}
 
 
-def _attn_ref(q, kv_of, b, heads, lq, d, scale, n_sets=1, chunk=1024):
+def _attn_ref(q, kv_of, b, heads, lq, d, scale, n_sets=1, chunk=1024, dt=BF16):
     """float64 attention; kv_of(i, s) -> (k, v) [lk, >= heads*d] of query batch i, set s.  With two sets each branch is
-    rounded to bf16 before the sum, as the kernel does."""
+    rounded to the storage type `dt` before the sum, as the kernel does."""
     c = heads * d
     out = torch.empty(b * lq, c, dtype=F64, device="cuda")
     for i in range(b):
@@ -286,15 +319,19 @@ def _attn_ref(q, kv_of, b, heads, lq, d, scale, n_sets=1, chunk=1024):
             o = torch.empty(heads, lq, d, dtype=F64, device="cuda")
             for r in range(0, lq, chunk):
                 o[:, r:r + chunk] = torch.softmax(qi[:, r:r + chunk] @ kh.transpose(1, 2) * scale, -1) @ vh
-            acc = acc + (o.to(BF16).to(F64) if n_sets == 2 else o)
+            acc = acc + (o.to(dt).to(F64) if n_sets == 2 else o)
         out[i * lq:(i + 1) * lq] = acc.transpose(0, 1).reshape(lq, c)
     return out
 
 
 def _attn_close(out, ref, n_sets=1):
-    # the xformers bf16 tolerance the reference's own kernel tests use (fmha/common.py:209-219); two bf16-rounded branches
-    # summed get the cross-view yardstick of test_kernels_gpu.py
-    torch.testing.assert_close(out.to(F64), ref, atol=2e-2 if n_sets == 1 else 3e-2, rtol=5e-3)
+    """The xformers tolerances the reference's own kernel tests use (fmha/common.py:209-219): bf16 atol 2e-2 / rtol 5e-3,
+    where two bf16-rounded branches summed get the cross-view yardstick of test_kernels_gpu.py (atol 3e-2); fp16 atol 4e-3 /
+    rtol 4e-4 for one set or several, whose f16 roundings the float64 reference repeats."""
+    if out.dtype == F16:
+        torch.testing.assert_close(out.to(F64), ref, atol=4e-3, rtol=4e-4)
+    else:
+        torch.testing.assert_close(out.to(F64), ref, atol=2e-2 if n_sets == 1 else 3e-2, rtol=5e-3)
 
 
 def _kv_index(entries):
@@ -303,8 +340,8 @@ def _kv_index(entries):
 
 @pytest.mark.parametrize("n_sets", [1, 2])
 @pytest.mark.parametrize("d", list(HEADS))
-@pytest.mark.parametrize("kernel", ATTN_KERNELS)
-def test_attention_multi_source(cuda_lib, monkeypatch, kernel, d, n_sets):
+@pytest.mark.parametrize("dt,kernel", ATTN_DT_KERNELS)
+def test_attention_multi_source(cuda_lib, monkeypatch, dt, kernel, d, n_sets):
     """K/V in three buffers (batch counts 6 / 3 / 3, row strides 2C / 2C / 3C), the view-sharded cross-view layout; kv_index
     entries (source << 24) | batch reach every source."""
     monkeypatch.setenv("MDB_ATTN_KERNEL", kernel)
@@ -313,17 +350,17 @@ def test_attention_multi_source(cuda_lib, monkeypatch, kernel, d, n_sets):
     c = heads * d
     b, lq, lk = 4, 201, 333
     scale = d ** -0.5
-    q = _bf(_randn(b * lq, c, g=g))
-    b0 = _bf(_randn(6 * lk, 2 * c, g=g))
-    b1 = _bf(_randn(3 * lk, 2 * c, g=g))
-    b2 = _bf(_randn(3 * lk, 3 * c, g=g))
+    q = _randn(b * lq, c, g=g).to(dt)
+    b0 = _randn(6 * lk, 2 * c, g=g).to(dt)
+    b1 = _randn(3 * lk, 2 * c, g=g).to(dt)
+    b2 = _randn(3 * lk, 3 * c, g=g).to(dt)
     srcs = [(b0[:, :c], b0[:, c:], 2 * c, 6), (b1[:, :c], b1[:, c:], 2 * c, 3), (b2[:, c:2 * c], b2[:, 2 * c:], 3 * c, 3)]
     if n_sets == 1:
         entries = [[(2, 1)], [(0, 5)], [(1, 2)], [(2, 0)]]
     else:
         entries = [[(0, 5), (2, 2)], [(1, 0), (0, 0)], [(2, 0), (1, 2)], [(0, 3), (2, 1)]]
     idx = _kv_index(entries)
-    out = Guarded(b * lq, c, ld=c + 16, col0=8)
+    out = Guarded(b * lq, c, dt, ld=c + 16, col0=8)
     ops.attention_multi(q, srcs, b=b, heads=heads, lq=lq, lk=lk, d=d, ldq=c, scale=scale, kv_index=idx, n_sets=n_sets,
                         out=out.out)
     out.check("multi-source")
@@ -333,11 +370,11 @@ def test_attention_multi_source(cuda_lib, monkeypatch, kernel, d, n_sets):
         k, v = srcs[src][:2]
         return k[j * lk:(j + 1) * lk], v[j * lk:(j + 1) * lk]
 
-    _attn_close(out.out, _attn_ref(q, kv_of, b, heads, lq, d, scale, n_sets), n_sets)
+    _attn_close(out.out, _attn_ref(q, kv_of, b, heads, lq, d, scale, n_sets, dt=dt), n_sets)
 
     # entries that all name source 0: bit for bit the single-buffer call
     e0 = [[(0, (3 * i + s) % 6) for s in range(n_sets)] for i in range(b)]
-    multi0 = Guarded(b * lq, c)
+    multi0 = Guarded(b * lq, c, dt)
     ops.attention_multi(q, srcs, b=b, heads=heads, lq=lq, lk=lk, d=d, ldq=c, scale=scale, kv_index=_kv_index(e0),
                         n_sets=n_sets, out=multi0.out)
     single0 = ops.attention(q, b0[:, :c], b0[:, c:], b=b, b_kv=6, heads=heads, lq=lq, lk=lk, d=d, ldq=c, ldk=2 * c,
@@ -346,10 +383,10 @@ def test_attention_multi_source(cuda_lib, monkeypatch, kernel, d, n_sets):
     assert torch.equal(multi0.out, single0)
 
     # three sources that are row ranges of one buffer: bit for bit the single-source call on the whole buffer
-    big = _bf(_randn(12 * lk, 2 * c, g=g))
+    big = _randn(12 * lk, 2 * c, g=g).to(dt)
     first = [0, 6, 9]
     slices = [(big[f * lk:(f + nb) * lk, :c], big[f * lk:(f + nb) * lk, c:], 2 * c, nb) for f, nb in zip(first, [6, 3, 3])]
-    split = Guarded(b * lq, c)
+    split = Guarded(b * lq, c, dt)
     ops.attention_multi(q, slices, b=b, heads=heads, lq=lq, lk=lk, d=d, ldq=c, scale=scale, kv_index=idx, n_sets=n_sets,
                         out=split.out)
     flat = torch.tensor([[first[s] + j for s, j in row] for row in entries], dtype=torch.int32, device="cuda")
@@ -360,20 +397,20 @@ def test_attention_multi_source(cuda_lib, monkeypatch, kernel, d, n_sets):
 
 
 @pytest.mark.parametrize("d", [40, 64])
-@pytest.mark.parametrize("kernel", ATTN_KERNELS)
-def test_attention_kv_batches_differ(cuda_lib, monkeypatch, kernel, d):
+@pytest.mark.parametrize("dt,kernel", ATTN_DT_KERNELS)
+def test_attention_kv_batches_differ(cuda_lib, monkeypatch, dt, kernel, d):
     """b_kv != b through kv_index with one set; queries read from a fused-QKV-style wide buffer."""
     monkeypatch.setenv("MDB_ATTN_KERNEL", kernel)
     g = _gen(8)
     heads = HEADS[d]
     c = heads * d
     b, b_kv, lq, lk = 5, 3, 333, 200
-    qbuf = _bf(_randn(b * lq, 3 * c, g=g))
+    qbuf = _randn(b * lq, 3 * c, g=g).to(dt)
     q = qbuf[:, c:2 * c]
-    kv = _bf(_randn(b_kv * lk, 2 * c, g=g))
+    kv = _randn(b_kv * lk, 2 * c, g=g).to(dt)
     sel = [2, 0, 1, 1, 2]
     idx = torch.tensor(sel, dtype=torch.int32, device="cuda")[:, None].contiguous()
-    out = Guarded(b * lq, c, ld=c + 64, col0=32)
+    out = Guarded(b * lq, c, dt, ld=c + 64, col0=32)
     ops.attention(q, kv, kv[:, c:], b=b, b_kv=b_kv, heads=heads, lq=lq, lk=lk, d=d, ldq=3 * c, ldk=2 * c, ldv=2 * c,
                   scale=d ** -0.5, kv_index=idx, out=out.out)
     out.check()
@@ -385,19 +422,28 @@ def test_attention_kv_batches_differ(cuda_lib, monkeypatch, kernel, d):
 def test_attention_multi_q_with_kv_index(cuda_lib, monkeypatch):
     """One K/V tile (lk <= 128) and more query tiles than SMs with kv_index and b_kv != b: multi-Q mode, against float64
     and bit for bit against one query tile per CTA."""
+    _multi_q_with_kv_index(monkeypatch, BF16)
+
+
+def test_attention_multi_q_with_kv_index_f16(cuda_lib, monkeypatch):
+    """test_attention_multi_q_with_kv_index for the f16 kernels."""
+    _multi_q_with_kv_index(monkeypatch, F16)
+
+
+def _multi_q_with_kv_index(monkeypatch, dt):
     monkeypatch.delenv("MDB_ATTN_KERNEL", raising=False)
     g = _gen(9)
     b, b_kv, heads, d, lq, lk = 6, 2, 8, 40, 1400, 77
     c = heads * d
     assert b * heads * ((lq + 127) // 128) > torch.cuda.get_device_properties(0).multi_processor_count
-    q = _bf(_randn(b * lq, c, g=g))
-    kv = _bf(_randn(b_kv * lk, 2 * c, g=g))
+    q = _randn(b * lq, c, g=g).to(dt)
+    kv = _randn(b_kv * lk, 2 * c, g=g).to(dt)
     sel = [1, 0, 1, 1, 0, 0]
     idx = torch.tensor(sel, dtype=torch.int32, device="cuda")[:, None].contiguous()
     outs = []
     for multiq in ("1", "0"):
         monkeypatch.setenv("MDB_ATTN_MULTIQ", multiq)
-        o = Guarded(b * lq, c, ld=c + 8, col0=8)
+        o = Guarded(b * lq, c, dt, ld=c + 8, col0=8)
         ops.attention(q, kv, kv[:, c:], b=b, b_kv=b_kv, heads=heads, lq=lq, lk=lk, d=d, ldq=c, ldk=2 * c, ldv=2 * c,
                       scale=d ** -0.5, kv_index=idx, out=o.out)
         o.check(f"MDB_ATTN_MULTIQ={multiq}")
@@ -408,15 +454,15 @@ def test_attention_multi_q_with_kv_index(cuda_lib, monkeypatch):
     assert torch.equal(outs[0], outs[1])
 
 
-@pytest.mark.parametrize("b,heads,d,l", [(2, 8, 40, 8400), (6, 8, 40, 5300)])
-def test_attention_long_self(cuda_lib, monkeypatch, b, heads, d, l):
+@pytest.mark.parametrize("dt,b,heads,d,l", with_dt([(2, 8, 40, 8400), (6, 8, 40, 5300)]))
+def test_attention_long_self(cuda_lib, monkeypatch, dt, b, heads, d, l):
     """The 'self' cross-view mode: one attention over the tokens of all six views (6 x 1400 at 224x400), and the
     424x800 level's 5300-token self-attention; fused-QKV input, output into a column slice."""
     monkeypatch.delenv("MDB_ATTN_KERNEL", raising=False)
     g = _gen(10)
     c = heads * d
-    qkv = _bf(_randn(b * l, 3 * c, g=g))
-    out = Guarded(b * l, c, ld=c + 16, col0=8)
+    qkv = _randn(b * l, 3 * c, g=g).to(dt)
+    out = Guarded(b * l, c, dt, ld=c + 16, col0=8)
     ops.attention(qkv, qkv[:, c:], qkv[:, 2 * c:], b=b, heads=heads, lq=l, lk=l, d=d, ldq=3 * c, ldk=3 * c, ldv=3 * c,
                   scale=d ** -0.5, out=out.out)
     out.check()
@@ -453,12 +499,18 @@ GN_CASES = ([(f"fused-{k}", v, {"MDB_GN_ROWS": "0"}, "gn_fused_kernel") for k, v
              ("odd-c96-ld0>c0", (2, 1400, 96, 32, 0), {"MDB_GN_ROWS": "0"}, "gn_stats_kernel")])
 
 
+GN_F16_NAMES = {"gn_rows_kernel": "gn_rows_f16_kernel", "gn_stats_kernel": "gn_stats_f16_kernel",
+                "gn_fused_kernel": "gn_fused_kernel"}  # gn_fused_kernel is one template for both element types
+
+
 @pytest.mark.parametrize("offset", [0, 16, 64, 256])
-@pytest.mark.parametrize("case,shape,env,kernel", GN_CASES, ids=[c[0] for c in GN_CASES])
-def test_groupnorm_kernels(cuda_lib, monkeypatch, case, shape, env, kernel, offset):
+@pytest.mark.parametrize("dt,case,shape,env,kernel", with_dt(GN_CASES, ids=[c[0] for c in GN_CASES]))
+def test_groupnorm_kernels(cuda_lib, monkeypatch, dt, case, shape, env, kernel, offset):
     """Each GroupNorm kernel, forced through its environment knobs, on inputs whose group means sit `offset` standard
     deviations away from zero; output into a column slice.  At 256 standard deviations a variance taken as
-    E[x^2] - mean^2 in fp32 is off by several percent on these group sizes; at 64 the error still hides in the bf16 output."""
+    E[x^2] - mean^2 in fp32 is off by several percent on these group sizes; at 64 the error still hides in the bf16 output.
+    f16 (mdb_groupnorm_f16): one f16 ulp of float64 (_close_f16).  At 256 standard deviations the f16 inputs sit around 128,
+    where their spacing is 1/8 of a standard deviation; the reference normalises the same stored values."""
     for k in ("MDB_GN_ROWS", "MDB_GN_ROWS_CLUSTER", "MDB_GN_TWO_KERNEL"):
         monkeypatch.delenv(k, raising=False)
     for k, v in env.items():
@@ -472,33 +524,35 @@ def test_groupnorm_kernels(cuda_lib, monkeypatch, case, shape, env, kernel, offs
     chan = _randn(c, g=g, scale=0.25 * sigma)  # per-channel means around the offset
 
     def make(rows, cols, ch):
-        return _bf(_randn(rows, cols, g=g, scale=sigma) + offset * sigma + ch)
+        return (_randn(rows, cols, g=g, scale=sigma) + offset * sigma + ch).to(dt)
 
     x0 = make(n * hw, c0 + pad, torch.cat([chan[:c0], torch.zeros(pad, device="cuda")]))[:, :c0]
     x1 = make(n * hw, c1, chan[c0:]) if c1 else None
     gamma = _randn(c, g=g)
     beta = _randn(c, g=g)
-    out = Guarded(n * hw, c, ld=c + 16, col0=8)
+    out = Guarded(n * hw, c, dt, ld=c + 16, col0=8)
     stats = torch.empty(max(n, 160) * groups * 2, dtype=F32, device="cuda")
+    fn = cuda_lib.mdb_groupnorm_f16 if dt == F16 else cuda_lib.mdb_groupnorm
+    names = {k: GN_F16_NAMES[k] if dt == F16 else k for k in GN_F16_NAMES}
 
     def run():
-        rc = cuda_lib.mdb_groupnorm(x0.data_ptr(), c0, c0 + pad, x1.data_ptr() if c1 else None, c1, c1, n, hw, groups, eps,
-                                    gamma.data_ptr(), beta.data_ptr(), int(silu), out.out.data_ptr(), out.ld,
-                                    stats.data_ptr(), torch.cuda.current_stream().cuda_stream)
+        rc = fn(x0.data_ptr(), c0, c0 + pad, x1.data_ptr() if c1 else None, c1, c1, n, hw, groups, eps, gamma.data_ptr(),
+                beta.data_ptr(), int(silu), out.out.data_ptr(), out.ld, stats.data_ptr(),
+                torch.cuda.current_stream().cuda_stream)
         assert rc == 0, cuda_lib.mdb_last_error()
 
     # the profiler now and then drops a kernel's record: profile again when no GroupNorm kernel shows up at all
     for _ in range(3):
         launched = _kernels_launched(run)
-        if any(k in launched for k in ("gn_rows_kernel", "gn_fused_kernel", "gn_stats_kernel")):
+        if any(k in launched for k in names.values()):
             break
-    assert kernel in launched, launched
+    assert names[kernel] in launched, launched
     out.check(case)
     full = x0.to(F64) if x1 is None else torch.cat([x0.to(F64), x1.to(F64)], 1)
     ref = F.group_norm(full.view(n, hw, c).permute(0, 2, 1), groups, gamma.to(F64), beta.to(F64), eps)
     if silu:
         ref = F.silu(ref)
-    _close_bf16(out.out, ref.permute(0, 2, 1).reshape(n * hw, c), case)
+    _close(out.out, ref.permute(0, 2, 1).reshape(n * hw, c), case)
 
 
 # ----------------------------------------------------------------------------------------- conv_direct, adaptive pool

@@ -13,10 +13,11 @@ from magicdrive_b200.models import BEVControlNetModel, UNet2DConditionModelMulti
 from magicdrive_b200.pipeline import BEVControlNetDenoiser  # noqa: E402
 from oracle import torch_oracle as O  # noqa: E402  (checker only)
 from tests.common import golden, rel_l2, tiny_configs, to_dev  # noqa: E402
-from tests.test_kernel_edges_gpu import ATTN_KERNELS, Guarded, _bf, _gen, _randn  # noqa: E402
+from tests.test_kernel_edges_gpu import ATTN_DT_KERNELS, ATTN_KERNELS, Guarded, _bf, _gen  # noqa: E402
+from tests.test_kernel_edges_gpu import _randn  # noqa: E402
 from tests.test_model_gpu import _bf16_yardstick, _check  # noqa: E402
 
-BF16, F64 = torch.bfloat16, torch.float64
+BF16, F16, F64 = torch.bfloat16, torch.float16, torch.float64
 DEV = "cuda"
 HEADS = {40: 4, 80: 2, 160: 2}
 CHAIN5 = {0: [1, 2], 1: [0, 3], 2: [0, 4], 3: [1], 4: [2]}
@@ -26,9 +27,9 @@ def _block_n(kernel, d):
     return {"tc2": 128 if d <= 64 else 64, "tc2d": 64, "tc": 128}[kernel]
 
 
-def _ref(q, kv_of, rows, heads, lq, d, scale):
-    """float64 sum over each query batch's present sets (kv_of(i) -> list of (k, v)), each set rounded to bf16 as the kernel
-    does; a batch without sets is zero."""
+def _ref(q, kv_of, rows, heads, lq, d, scale, dt=BF16):
+    """float64 sum over each query batch's present sets (kv_of(i) -> list of (k, v)), each set rounded to the storage type
+    `dt` as the kernel does; a batch without sets is zero."""
     c = heads * d
     out = torch.zeros(len(rows) * lq, c, dtype=F64, device=DEV)
     for i in range(len(rows)):
@@ -37,14 +38,17 @@ def _ref(q, kv_of, rows, heads, lq, d, scale):
         for k, v in kv_of(i):
             kh = k[:, :c].to(F64).reshape(-1, heads, d).transpose(0, 1)
             vh = v[:, :c].to(F64).reshape(-1, heads, d).transpose(0, 1)
-            acc = acc + (torch.softmax(qi @ kh.transpose(1, 2) * scale, -1) @ vh).to(BF16).to(F64)
+            acc = acc + (torch.softmax(qi @ kh.transpose(1, 2) * scale, -1) @ vh).to(dt).to(F64)
         if torch.is_tensor(acc):
             out[i * lq:(i + 1) * lq] = acc.transpose(0, 1).reshape(lq, c)
     return out
 
 
 def _close(out, ref, n_sets):
-    torch.testing.assert_close(out.to(F64), ref, atol=2e-2 if n_sets == 1 else 3e-2 + 4e-3 * n_sets, rtol=5e-3)
+    if out.dtype == F16:  # xformers' fp16 tolerance (test_kernel_edges_gpu._attn_close)
+        torch.testing.assert_close(out.to(F64), ref, atol=4e-3, rtol=4e-4)
+    else:
+        torch.testing.assert_close(out.to(F64), ref, atol=2e-2 if n_sets == 1 else 3e-2 + 4e-3 * n_sets, rtol=5e-3)
 
 
 def _sources(g, c, lk, n_src):
@@ -124,10 +128,11 @@ def test_attention_empty_slots_are_bitwise_absent(cuda_lib, monkeypatch, kernel,
 
 
 @pytest.mark.parametrize("d", list(HEADS))
-@pytest.mark.parametrize("kernel", ATTN_KERNELS)
-def test_attention_kv_len(cuda_lib, monkeypatch, kernel, d):
+@pytest.mark.parametrize("dt,kernel", ATTN_DT_KERNELS)
+def test_attention_kv_len(cuda_lib, monkeypatch, dt, kernel, d):
     """Per-batch key counts 0, 1, below one key tile, BN - 1 / BN / BN + 1, lk, and out-of-range values the kernel clamps;
-    one set and three sets with an empty slot."""
+    one set and three sets with an empty slot.  lk = 2 BN + 37 puts the 128-key tiles (d <= 64) past the KVRES kernel's
+    256 keys: the varlen kernel without resident key tiles, in bf16 and f16."""
     monkeypatch.setenv("MDB_ATTN_KERNEL", kernel)
     g = _gen(10)
     heads = HEADS[d]
@@ -137,11 +142,11 @@ def test_attention_kv_len(cuda_lib, monkeypatch, kernel, d):
     lens = [0, 1, 17, bn - 1, bn, bn + 1, lk, -5, lk + 40]
     b = len(lens)
     scale = d ** -0.5
-    q = _bf(_randn(b * lq, c, g=g))
-    kv = _bf(_randn(b * lk, 2 * c, g=g))
+    q = _randn(b * lq, c, g=g).to(dt)
+    kv = _randn(b * lk, 2 * c, g=g).to(dt)
     kv_len = torch.tensor(lens, dtype=torch.int32, device=DEV)
     eff = [min(max(x, 0), lk) for x in lens]
-    out = Guarded(b * lq, c, ld=c + 16, col0=8)
+    out = Guarded(b * lq, c, dt, ld=c + 16, col0=8)
     ops.attention(q, kv, kv[:, c:], b=b, heads=heads, lq=lq, lk=lk, d=d, ldq=c, ldk=2 * c, ldv=2 * c, scale=scale,
                   kv_len=kv_len, out=out.out)
     out.check("kv_len")
@@ -149,10 +154,10 @@ def test_attention_kv_len(cuda_lib, monkeypatch, kernel, d):
     def kv_of(i):
         return [(kv[i * lk:i * lk + eff[i], :c], kv[i * lk:i * lk + eff[i], c:])] if eff[i] else []
 
-    _close(out.out, _ref(q, kv_of, lens, heads, lq, d, scale), 1)
+    _close(out.out, _ref(q, kv_of, lens, heads, lq, d, scale, dt), 1)
     # three sets of which one empty, each set cut to its query batch's key count
     rows = [[(0, (i + 1) % b), None, (0, (i + 4) % b)] for i in range(b)]
-    out3 = Guarded(b * lq, c)
+    out3 = Guarded(b * lq, c, dt)
     ops.attention(q, kv, kv[:, c:], b=b, heads=heads, lq=lq, lk=lk, d=d, ldq=c, ldk=2 * c, ldv=2 * c, scale=scale,
                   kv_index=_kv_index(rows), n_sets=3, kv_len=kv_len, out=out3.out)
     out3.check("kv_len, three sets")
@@ -160,7 +165,7 @@ def test_attention_kv_len(cuda_lib, monkeypatch, kernel, d):
     def kv3(i):
         return [(kv[e[1] * lk:e[1] * lk + eff[i], :c], kv[e[1] * lk:e[1] * lk + eff[i], c:]) for e in rows[i] if e and eff[i]]
 
-    _close(out3.out, _ref(q, kv3, rows, heads, lq, d, scale), 3)
+    _close(out3.out, _ref(q, kv3, rows, heads, lq, d, scale, dt), 3)
     # kv_len = lk everywhere is bit for bit the call without kv_len
     full = ops.attention(q, kv, kv[:, c:], b=b, heads=heads, lq=lq, lk=lk, d=d, ldq=c, ldk=2 * c, ldv=2 * c, scale=scale,
                          kv_len=torch.full((b,), lk, dtype=torch.int32, device=DEV))

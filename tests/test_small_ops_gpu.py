@@ -37,14 +37,14 @@ pytestmark = pytest.mark.gpu
 from magicdrive_b200 import _lib, ops  # noqa: E402
 from oracle import input_prep as OP  # noqa: E402  (checker only)
 from tests.common import record  # noqa: E402
-from tests.test_kernel_edges_gpu import _FILL, BF16, F32, F64, G, _bf, _gen  # noqa: E402
+from tests.test_kernel_edges_gpu import _FILL, BF16, F16, F32, F64, G, _bf, _gen, with_dt  # noqa: E402
 from tests.test_kernel_edges_gpu import Guarded as _Guarded  # noqa: E402
 from tests.test_kernel_edges_gpu import _attn_close, _close, _close_f32  # noqa: E402
 
 I32, I64, U8 = torch.int32, torch.int64, torch.uint8
 INVALID, UNSUPPORTED = -1, -3
 _FILL_INT = {I32: (I32, 0x5AA5A55A), I64: (I64, 0x5AA5A55A5AA5A55A), U8: (U8, 0xA5)}  # values no kernel here writes
-_BITS = {BF16: torch.int16, F32: torch.int32}
+_BITS = {BF16: torch.int16, F16: torch.int16, F32: torch.int32}
 WORST = {}  # operator -> largest measured |err| / bound
 
 
@@ -174,16 +174,19 @@ def test_nhwc_to_nchw_bitwise(cuda_lib, c, n, h, w, out_dtype):
 
 
 @pytest.mark.parametrize("repeat", [1, 2])
-@pytest.mark.parametrize("x_dtype", [F32, BF16], ids=["f32", "bf16"])
+@pytest.mark.parametrize("x_dtype", [F32, BF16, F16], ids=["f32", "bf16", "f16"])
 @pytest.mark.parametrize("pix", [12 * 28 * 50, 1001])
 def test_pack_latents_bitwise(cuda_lib, pix, x_dtype, repeat):
+    """mdb_pack_latents from fp32 / bf16, and mdb_pack_latents_f16 (an fp16 model's conv_in operand) from an f16 source,
+    which it copies without a conversion (its fp32 source is test_fp16_kernels_gpu.py's)."""
     cin, cpad = 4, 64
     x = (torch.randn(pix, cin, device="cuda", generator=_gen(5)) * 3).to(x_dtype)
-    out = Guarded(repeat * pix, cpad, BF16)
-    _lib_ok(cuda_lib.mdb_pack_latents(x.data_ptr(), int(x_dtype == F32), pix, cin, cpad, repeat, out.out.data_ptr(), _st()),
-            "pack_latents")
+    odt = F16 if x_dtype == F16 else BF16
+    fn = cuda_lib.mdb_pack_latents_f16 if x_dtype == F16 else cuda_lib.mdb_pack_latents
+    out = Guarded(repeat * pix, cpad, odt)
+    _lib_ok(fn(x.data_ptr(), int(x_dtype == F32), pix, cin, cpad, repeat, out.out.data_ptr(), _st()), "pack_latents")
     out.check("pack_latents")
-    _same(out.out, F.pad(x.to(BF16), (0, cpad - cin)).repeat(repeat, 1), "pack_latents")
+    _same(out.out, F.pad(x.to(odt), (0, cpad - cin)).repeat(repeat, 1), "pack_latents")
 
 
 # ------------------------------------------------------------------------------------------------------ conversions
@@ -392,16 +395,19 @@ LINEAR_SMALL = [
 ]
 
 
-@pytest.mark.parametrize("m,n,k,dw,di,do,bias,pre,post", LINEAR_SMALL)
-def test_linear_small(cuda_lib, m, n, k, dw, di, do, bias, pre, post):
+@pytest.mark.parametrize("wdt,m,n,k,dw,di,do,bias,pre,post", with_dt(LINEAR_SMALL))
+def test_linear_small(cuda_lib, wdt, m, n, k, dw, di, do, bias, pre, post):
+    """fp32 activations times bf16 weights (mdb_linear_small) or f16 weights (mdb_linear_small_f16, fp16 models).  The
+    bound is one of fp32 arithmetic on the weights as stored, so it holds for either weight type."""
     g = _gen(11)
     ldw, ldi, ldo = k + dw, k + di, n + do
     xin = torch.randn(m, ldi, device="cuda", generator=g) * 2
-    wbuf = _bf(torch.randn(n, ldw, device="cuda", generator=g) / math.sqrt(k))
+    wbuf = (torch.randn(n, ldw, device="cuda", generator=g) / math.sqrt(k)).to(wdt)
     b = torch.randn(n, device="cuda", generator=g) if bias else None
     out = Guarded(m, n, F32, ld=ldo, col0=do // 2)  # guard columns on both sides when ldo > n
-    rc = cuda_lib.mdb_linear_small(xin.data_ptr(), m, k, ldi, wbuf.data_ptr(), ldw, b.data_ptr() if bias else None, n,
-                                   int(pre), int(post), out.out.data_ptr(), ldo, _st())
+    fn = cuda_lib.mdb_linear_small_f16 if wdt == F16 else cuda_lib.mdb_linear_small
+    rc = fn(xin.data_ptr(), m, k, ldi, wbuf.data_ptr(), ldw, b.data_ptr() if bias else None, n, int(pre), int(post),
+            out.out.data_ptr(), ldo, _st())
     _lib_ok(rc, "linear_small")
     out.check(f"linear_small m={m} n={n} k={k}")
     y, bound = _linear_small_ref(xin[:, :k], wbuf[:, :k], b, pre, post)
