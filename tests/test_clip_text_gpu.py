@@ -12,6 +12,7 @@ pytestmark = pytest.mark.gpu
 
 from magicdrive_b200 import _lib, arch, models, ops  # noqa: E402
 from oracle.clip_text import clip_text_forward, draw_weights  # noqa: E402  (checker only)
+from tests.attention_model import attention_model, check_model  # noqa: E402
 from tests.common import golden, record, rel_l2, tiny_configs, tiny_state_dicts  # noqa: E402
 from tests.test_kernel_edges_gpu import BF16, F32, F64, Guarded, _bf, _close_bf16, _gen, _randn  # noqa: E402
 
@@ -22,11 +23,10 @@ HEADS = 12
 
 # ------------------------------------------------------------------------------------------------ causal attention
 def _causal_ref(qkv, b, l, d):
+    """float64 causal attention over a fused-QKV buffer and its error model (tests/attention_model.py)."""
     c = HEADS * d
-    x = qkv.to(F64).reshape(b, l, 3, HEADS, d).permute(2, 0, 3, 1, 4)  # [3, b, heads, l, d]
-    s = x[0] @ x[1].transpose(-1, -2) * d ** -0.5
-    s = s + torch.full((l, l), float("-inf"), dtype=F64, device=DEV).triu(1)
-    return (torch.softmax(s, -1) @ x[2]).transpose(1, 2).reshape(b * l, c)
+    return attention_model(qkv, lambda i: [(qkv[i * l:(i + 1) * l, c:2 * c], qkv[i * l:(i + 1) * l, 2 * c:])], b, HEADS, l,
+                           d, d ** -0.5, BF16, causal=True)
 
 
 def _causal(qkv, b, l, d, out):
@@ -52,8 +52,7 @@ def test_attention_causal(cuda_lib, monkeypatch, kernel, d, multiq):
             out = Guarded(b * l, c, ld=c + 16, col0=8)
             _causal(qkv, b, l, d, out.out)
             out.check(f"b={b} L={l}")
-            torch.testing.assert_close(out.out.to(F64), _causal_ref(qkv, b, l, d), atol=2e-2, rtol=5e-3,
-                                       msg=lambda m: f"b={b} L={l}: {m}")
+            check_model(out.out, _causal_ref(qkv, b, l, d), f"b={b} L={l}")
             if multiq == "0":
                 monkeypatch.setenv("MDB_ATTN_MULTIQ", "1")
                 again = _causal(qkv, b, l, d, None)

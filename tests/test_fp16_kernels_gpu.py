@@ -1,6 +1,6 @@
 """The f16 instantiations of the denoising step's kernels (models with fp16 parameters): GEMM / implicit-GEMM convolution with
-every epilogue the step uses, fused attention, GroupNorm(+SiLU) and the glue, each against float64 (attention against fp32,
-within xformers' fp16 tolerance) and every output guard-banded as in test_kernel_edges_gpu.py, which runs the same kernels
+every epilogue the step uses, fused attention, GroupNorm(+SiLU) and the glue, each against float64 (attention under the error
+model of tests/attention_model.py) and every output guard-banded as in test_kernel_edges_gpu.py, which runs the same kernels
 at the tiling edges in both element types.  Here: fp16's own range (overflow to inf, subnormal results and operands), and
 the operators' refusal of operands whose element types disagree."""
 import math
@@ -14,6 +14,7 @@ pytestmark = pytest.mark.gpu
 
 from magicdrive_b200 import f16_ops, ops  # noqa: E402
 from magicdrive_b200.params import pack_geglu  # noqa: E402
+from tests.attention_model import attention_model, check_model  # noqa: E402
 from tests.test_kernel_edges_gpu import BF16, F16, F32, F64, Guarded, _close_f16  # noqa: E402
 
 
@@ -145,18 +146,11 @@ def test_f16_rejections(cuda_lib):
 
 
 # ---------------------------------------------------------------------------------------------------------- attention
-def _attn_ref(q, k, v, b, bkv, heads, lq, lk, d, scale, n_keys=None):
-    qh = q.float().reshape(b, lq, heads, d).transpose(1, 2)
-    kh = k.float().reshape(bkv, lk, heads, d).transpose(1, 2)
-    vh = v.float().reshape(bkv, lk, heads, d).transpose(1, 2)
-    s = qh @ kh.transpose(-1, -2) * scale
-    if n_keys is not None:
-        s = s.masked_fill(torch.arange(lk, device="cuda")[None, None, None] >= n_keys[:, None, None, None], float("-inf"))
-    return (torch.softmax(s, -1) @ vh).transpose(1, 2).reshape(b * lq, heads * d)
-
-
-def _xformers_close(out, ref, what=""):
-    assert torch.allclose(out.float(), ref, atol=4e-3, rtol=4e-4), f"{what}: max err {(out.float() - ref).abs().max().item():.3e}"
+def _attn_ref(q, k, v, b, heads, lq, lk, d, scale, n_keys=None):
+    """The float64 attention of q [b*lq, C] over k / v [b*lk, C] (the first n_keys[i] keys of batch i) and its error model
+    (tests/attention_model.py)."""
+    n = [lk] * b if n_keys is None else n_keys.tolist()
+    return attention_model(q, lambda i: [(k[i * lk:i * lk + n[i]], v[i * lk:i * lk + n[i]])], b, heads, lq, d, scale, F16)
 
 
 @pytest.mark.parametrize("d", [32, 40, 64, 80, 160])
@@ -169,7 +163,7 @@ def test_attention(cuda_lib, d, lq, lk):
     ops.attention(q, k, v, b=b, heads=heads, lq=lq, lk=lk, d=d, ldq=heads * d, ldk=heads * d, ldv=heads * d,
                   scale=d ** -0.5, out=o.out)
     o.check(f"attention d={d}")
-    _xformers_close(o.out, _attn_ref(q, k, v, b, b, heads, lq, lk, d, d ** -0.5), f"attention d={d}")
+    check_model(o.out, _attn_ref(q, k, v, b, heads, lq, lk, d, d ** -0.5), f"attention d={d}")
 
 
 @pytest.mark.parametrize("d", [40, 64, 80])
@@ -195,11 +189,9 @@ def test_attention_add_sets_with_empty_slots(cuda_lib, d):
             continue
         t = qkv.reshape(b, L, 3 * C)
         qi = t[i, :, :C].contiguous()
-        ref = torch.zeros(L, C, device="cuda")
-        for j in present:
-            kj, vj = t[j, :, C:2 * C].contiguous(), t[j, :, 2 * C:].contiguous()
-            ref = ref + _attn_ref(qi, kj, vj, 1, 1, heads, L, L, d, d ** -0.5).half().float()
-        _xformers_close(o3.reshape(b, L, C)[i], ref, f"add mode d={d} row {i}")
+        kvs = [(t[j, :, C:2 * C], t[j, :, 2 * C:]) for j in present]
+        check_model(o3.reshape(b, L, C)[i], attention_model(qi, lambda _: kvs, 1, heads, L, d, d ** -0.5, F16),
+                    f"add mode d={d} row {i}")
 
 
 @pytest.mark.parametrize("d", [40, 80, 160])
@@ -220,8 +212,7 @@ def test_attention_kv_len_resident_and_multi_q_bitwise(cuda_lib, d):
         oi = ops.attention(q.reshape(b, lq, C)[i].contiguous(), kvi, kvi[:, C:], lk=n, **dict(kw, b=1))
         torch.cuda.synchronize()
         assert torch.equal(o.reshape(b, lq, C)[i], oi), (d, i)
-    ref = _attn_ref(q, kv[:, :C].contiguous(), kv[:, C:].contiguous(), b, b, heads, lq, cap, d, d ** -0.5, lens.long())
-    _xformers_close(o, ref, f"kv_len d={d}")
+    check_model(o, _attn_ref(q, kv[:, :C], kv[:, C:], b, heads, lq, cap, d, d ** -0.5, lens), f"kv_len d={d}")
     # multi-Q: one key tile (lk <= BN), more query tiles than SMs hold at once
     lk = 64
     kv2 = kv[: b * lk]

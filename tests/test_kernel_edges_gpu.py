@@ -20,6 +20,7 @@ import torch.nn.functional as F
 pytestmark = pytest.mark.gpu
 
 from magicdrive_b200 import ops  # noqa: E402
+from tests.attention_model import attention_model, check_model  # noqa: E402
 
 BF16, F16, F32, F64 = torch.bfloat16, torch.float16, torch.float32, torch.float64
 G = 128  # guard rows before and after every output: one full GEMM M tile
@@ -304,34 +305,15 @@ ATTN_DT_KERNELS = with_dt(ATTN_KERNELS, f16=("tc2",))
 HEADS = {32: 2, 40: 8, 64: 2, 80: 4, 160: 2}
 
 
-def _attn_ref(q, kv_of, b, heads, lq, d, scale, n_sets=1, chunk=1024, dt=BF16):
-    """float64 attention; kv_of(i, s) -> (k, v) [lk, >= heads*d] of query batch i, set s.  With two sets each branch is
-    rounded to the storage type `dt` before the sum, as the kernel does."""
-    c = heads * d
-    out = torch.empty(b * lq, c, dtype=F64, device="cuda")
-    for i in range(b):
-        qi = q[i * lq:(i + 1) * lq, :c].to(F64).reshape(lq, heads, d).transpose(0, 1)
-        acc = 0
-        for s in range(n_sets):
-            k, v = kv_of(i, s)
-            kh = k[:, :c].to(F64).reshape(-1, heads, d).transpose(0, 1)
-            vh = v[:, :c].to(F64).reshape(-1, heads, d).transpose(0, 1)
-            o = torch.empty(heads, lq, d, dtype=F64, device="cuda")
-            for r in range(0, lq, chunk):
-                o[:, r:r + chunk] = torch.softmax(qi[:, r:r + chunk] @ kh.transpose(1, 2) * scale, -1) @ vh
-            acc = acc + (o.to(dt).to(F64) if n_sets == 2 else o)
-        out[i * lq:(i + 1) * lq] = acc.transpose(0, 1).reshape(lq, c)
-    return out
+def _attn_ref(q, kv_of, b, heads, lq, d, scale, n_sets=1, chunk=512, dt=BF16):
+    """The float64 attention and its error model (tests/attention_model.py); kv_of(i, s) -> (k, v) [lk, >= heads*d] of
+    query batch i, set s."""
+    return attention_model(q, lambda i: [kv_of(i, s) for s in range(n_sets)], b, heads, lq, d, scale, dt, chunk=chunk)
 
 
-def _attn_close(out, ref, n_sets=1):
-    """The xformers tolerances the reference's own kernel tests use (fmha/common.py:209-219): bf16 atol 2e-2 / rtol 5e-3,
-    where two bf16-rounded branches summed get the cross-view yardstick of test_kernels_gpu.py (atol 3e-2); fp16 atol 4e-3 /
-    rtol 4e-4 for one set or several, whose f16 roundings the float64 reference repeats."""
-    if out.dtype == F16:
-        torch.testing.assert_close(out.to(F64), ref, atol=4e-3, rtol=4e-4)
-    else:
-        torch.testing.assert_close(out.to(F64), ref, atol=2e-2 if n_sets == 1 else 3e-2, rtol=5e-3)
+def _attn_close(out, model):
+    """Both criteria of the error model of the kernel's roundings (tests/attention_model.py)."""
+    check_model(out, model)
 
 
 def _kv_index(entries):
@@ -370,7 +352,7 @@ def test_attention_multi_source(cuda_lib, monkeypatch, dt, kernel, d, n_sets):
         k, v = srcs[src][:2]
         return k[j * lk:(j + 1) * lk], v[j * lk:(j + 1) * lk]
 
-    _attn_close(out.out, _attn_ref(q, kv_of, b, heads, lq, d, scale, n_sets, dt=dt), n_sets)
+    _attn_close(out.out, _attn_ref(q, kv_of, b, heads, lq, d, scale, n_sets, dt=dt))
 
     # entries that all name source 0: bit for bit the single-buffer call
     e0 = [[(0, (3 * i + s) % 6) for s in range(n_sets)] for i in range(b)]
@@ -415,7 +397,7 @@ def test_attention_kv_batches_differ(cuda_lib, monkeypatch, dt, kernel, d):
                   scale=d ** -0.5, kv_index=idx, out=out.out)
     out.check()
     ref = _attn_ref(q, lambda i, s: (kv[sel[i] * lk:(sel[i] + 1) * lk, :c], kv[sel[i] * lk:(sel[i] + 1) * lk, c:]),
-                    b, heads, lq, d, d ** -0.5)
+                    b, heads, lq, d, d ** -0.5, dt=dt)
     _attn_close(out.out, ref)
 
 
@@ -449,7 +431,7 @@ def _multi_q_with_kv_index(monkeypatch, dt):
         o.check(f"MDB_ATTN_MULTIQ={multiq}")
         outs.append(o.out)
     ref = _attn_ref(q, lambda i, s: (kv[sel[i] * lk:(sel[i] + 1) * lk, :c], kv[sel[i] * lk:(sel[i] + 1) * lk, c:]),
-                    b, heads, lq, d, d ** -0.5)
+                    b, heads, lq, d, d ** -0.5, dt=dt)
     _attn_close(outs[0], ref)
     assert torch.equal(outs[0], outs[1])
 
@@ -467,7 +449,7 @@ def test_attention_long_self(cuda_lib, monkeypatch, dt, b, heads, d, l):
                   scale=d ** -0.5, out=out.out)
     out.check()
     ref = _attn_ref(qkv, lambda i, s: (qkv[i * l:(i + 1) * l, c:2 * c], qkv[i * l:(i + 1) * l, 2 * c:]), b, heads, l, d,
-                    d ** -0.5)
+                    d ** -0.5, dt=dt)
     _attn_close(out.out, ref)
 
 

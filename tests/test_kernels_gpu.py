@@ -8,6 +8,7 @@ import torch.nn.functional as F
 pytestmark = pytest.mark.gpu
 
 from magicdrive_b200 import ops  # noqa: E402
+from tests.attention_model import attention_model, check_model  # noqa: E402
 
 
 def _bf(x):
@@ -190,6 +191,12 @@ def test_layernorm(cuda_lib, c):
 ATTN_KERNELS = ["tc2", "tc2d", "tc"]  # key-tile width: per head dim (default) | 64 keys | 128 keys
 
 
+def _attn_model(q, k, v, b, heads, lq, lk, d, scale):
+    """float64 attention of q [b*lq, C] over k / v [b*lk, C] (row strides free) and its error model
+    (tests/attention_model.py)."""
+    return attention_model(q, lambda i: [(k[i * lk:(i + 1) * lk], v[i * lk:(i + 1) * lk])], b, heads, lq, d, scale, torch.bfloat16)
+
+
 def _pick_attention_kernel(monkeypatch, kernel):
     monkeypatch.delenv("MDB_ATTN_LEGACY", raising=False)
     monkeypatch.setenv("MDB_ATTN_KERNEL", kernel)
@@ -208,13 +215,7 @@ def test_attention(cuda_lib, monkeypatch, d, heads, lq, lk, kernel):
     v = _bf(torch.randn(b * lk, c, device="cuda", generator=g))
     scale = d ** -0.5
     out = ops.attention(q, k, v, b=b, heads=heads, lq=lq, lk=lk, d=d, ldq=c, ldk=c, ldv=c, scale=scale)
-    qh = q.float().reshape(b, lq, heads, d).transpose(1, 2)
-    kh = k.float().reshape(b, lk, heads, d).transpose(1, 2)
-    vh = v.float().reshape(b, lk, heads, d).transpose(1, 2)
-    ref = torch.softmax(qh @ kh.transpose(-1, -2) * scale, -1) @ vh
-    ref = ref.transpose(1, 2).reshape(b * lq, c)
-    # the xformers bf16 tolerance the reference's own kernel tests use (fmha/common.py:209-219): atol 2e-2 rtol 5e-3
-    torch.testing.assert_close(out.float(), ref, atol=2e-2, rtol=5e-3)
+    check_model(out, _attn_model(q, k, v, b, heads, lq, lk, d, scale))
 
 
 @pytest.mark.parametrize("b,heads,d,lq,lk", [(12, 8, 40, 1400, 98), (12, 8, 40, 1337, 128), (12, 8, 40, 1400, 40), (30, 2, 32, 1400, 77),
@@ -233,11 +234,7 @@ def test_attention_multi_q_tiles_per_cta(cuda_lib, monkeypatch, b, heads, d, lq,
     out = ops.attention(q, k, v, b=b, heads=heads, lq=lq, lk=lk, d=d, ldq=c, ldk=c, ldv=c, scale=scale)
     monkeypatch.setenv("MDB_ATTN_MULTIQ", "0")
     one = ops.attention(q, k, v, b=b, heads=heads, lq=lq, lk=lk, d=d, ldq=c, ldk=c, ldv=c, scale=scale)
-    qh = q.float().reshape(b, lq, heads, d).transpose(1, 2)
-    kh = k.float().reshape(b, lk, heads, d).transpose(1, 2)
-    vh = v.float().reshape(b, lk, heads, d).transpose(1, 2)
-    ref = (torch.softmax(qh @ kh.transpose(-1, -2) * scale, -1) @ vh).transpose(1, 2).reshape(b * lq, c)
-    torch.testing.assert_close(out.float(), ref, atol=2e-2, rtol=5e-3)
+    check_model(out, _attn_model(q, k, v, b, heads, lq, lk, d, scale))
     assert torch.equal(out, one)
 
 
@@ -257,11 +254,7 @@ def test_attention_growing_scores(cuda_lib, monkeypatch, d, heads, lq, lk, kerne
     v = _bf(torch.randn(b * lk, c, device="cuda", generator=g))
     scale = d ** -0.5
     out = ops.attention(q, k, v, b=b, heads=heads, lq=lq, lk=lk, d=d, ldq=c, ldk=c, ldv=c, scale=scale)
-    qh = q.float().reshape(b, lq, heads, d).transpose(1, 2)
-    kh = k.float().reshape(b, lk, heads, d).transpose(1, 2)
-    vh = v.float().reshape(b, lk, heads, d).transpose(1, 2)
-    ref = (torch.softmax(qh @ kh.transpose(-1, -2) * scale, -1) @ vh).transpose(1, 2).reshape(b * lq, c)
-    torch.testing.assert_close(out.float(), ref, atol=2e-2, rtol=5e-3)
+    check_model(out, _attn_model(q, k, v, b, heads, lq, lk, d, scale))
 
 
 @pytest.mark.parametrize("kernel", ATTN_KERNELS)
@@ -280,15 +273,10 @@ def test_attention_two_sets_cross_view(cuda_lib, monkeypatch, kernel, l, heads, 
                        dtype=torch.int32, device="cuda")
     out = ops.attention(q, k, v, b=b, heads=heads, lq=l, lk=l, d=d, ldq=3 * c, ldk=3 * c, ldv=3 * c, scale=d ** -0.5,
                         kv_index=idx, n_sets=2)
-    qh = q.float().reshape(b, l, heads, d).transpose(1, 2)
-    kh = k.float().reshape(b, l, heads, d).transpose(1, 2)
-    vh = v.float().reshape(b, l, heads, d).transpose(1, 2)
-    ref = 0
-    for s in range(2):
-        sel = idx[:, s].long()
-        ref = ref + torch.softmax(qh @ kh[sel].transpose(-1, -2) * d ** -0.5, -1) @ vh[sel]
-    ref = ref.transpose(1, 2).reshape(b * l, c)
-    torch.testing.assert_close(out.float(), ref, atol=3e-2, rtol=5e-3)
+    sets = idx.tolist()
+    m = attention_model(q, lambda i: [(k[j * l:(j + 1) * l], v[j * l:(j + 1) * l]) for j in sets[i]], b, heads, l, d,
+                        d ** -0.5, torch.bfloat16)
+    check_model(out, m)
 
 
 def test_pointwise_and_embeddings(cuda_lib):

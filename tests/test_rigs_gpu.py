@@ -12,6 +12,7 @@ from magicdrive_b200 import arch, ops  # noqa: E402
 from magicdrive_b200.models import BEVControlNetModel, UNet2DConditionModelMultiview  # noqa: E402
 from magicdrive_b200.pipeline import BEVControlNetDenoiser  # noqa: E402
 from oracle import torch_oracle as O  # noqa: E402  (checker only)
+from tests.attention_model import attention_model, check_model  # noqa: E402
 from tests.common import golden, rel_l2, tiny_configs, to_dev  # noqa: E402
 from tests.test_kernel_edges_gpu import ATTN_DT_KERNELS, ATTN_KERNELS, Guarded, _bf, _gen  # noqa: E402
 from tests.test_kernel_edges_gpu import _randn  # noqa: E402
@@ -28,27 +29,13 @@ def _block_n(kernel, d):
 
 
 def _ref(q, kv_of, rows, heads, lq, d, scale, dt=BF16):
-    """float64 sum over each query batch's present sets (kv_of(i) -> list of (k, v)), each set rounded to the storage type
-    `dt` as the kernel does; a batch without sets is zero."""
-    c = heads * d
-    out = torch.zeros(len(rows) * lq, c, dtype=F64, device=DEV)
-    for i in range(len(rows)):
-        qi = q[i * lq:(i + 1) * lq, :c].to(F64).reshape(lq, heads, d).transpose(0, 1)
-        acc = 0
-        for k, v in kv_of(i):
-            kh = k[:, :c].to(F64).reshape(-1, heads, d).transpose(0, 1)
-            vh = v[:, :c].to(F64).reshape(-1, heads, d).transpose(0, 1)
-            acc = acc + (torch.softmax(qi @ kh.transpose(1, 2) * scale, -1) @ vh).to(dt).to(F64)
-        if torch.is_tensor(acc):
-            out[i * lq:(i + 1) * lq] = acc.transpose(0, 1).reshape(lq, c)
-    return out
+    """The float64 sum over each query batch's present sets (kv_of(i) -> list of (k, v)) and its error model
+    (tests/attention_model.py); a batch without sets is zero."""
+    return attention_model(q, kv_of, len(rows), heads, lq, d, scale, dt)
 
 
-def _close(out, ref, n_sets):
-    if out.dtype == F16:  # xformers' fp16 tolerance (test_kernel_edges_gpu._attn_close)
-        torch.testing.assert_close(out.to(F64), ref, atol=4e-3, rtol=4e-4)
-    else:
-        torch.testing.assert_close(out.to(F64), ref, atol=2e-2 if n_sets == 1 else 3e-2 + 4e-3 * n_sets, rtol=5e-3)
+def _close(out, model, n_sets):
+    check_model(out, model, f"{n_sets} sets")
 
 
 def _sources(g, c, lk, n_src):
