@@ -333,6 +333,33 @@ int mdb_prepare_boxes(const float* boxes, int box_dim, const long long* labels, 
                       long long* out_classes, unsigned char* out_masks, int* out_counts, void* stream);
 int mdb_camera_param(const float* intrinsics, const float* lidar2camera, int n, float* out, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * 3D-box overlays (demo/helper.py:197-307: visualize_camera, show_box_on_views, draw_box_on_imgs with thickness 1):
+ * each view with its boxes drawn as OpenCV draws them, byte for byte.
+ * mdb_project_boxes: per (scene, view), the boxes whose 8 corners (of the box shifted down by dz/2, mmdet3d order, fp32)
+ *   all lie in front of the camera (z > 0 in float64 after `transform`), ordered far to near by their smallest z (a
+ *   stable order: exact ties keep box order, which numpy's argsort does not promise beyond 16 boxes).
+ *   boxes: fp32 [sum n_s, box_dim >= 7] (x, y, z, dx, dy, dz, yaw, ...), bottom-centred; sincos: fp32 [sum n_s, 2],
+ *   sin and cos of each yaw as the caller computes them; labels: int64 [sum n_s]; box_offsets: int32 [n_scenes + 1];
+ *   transforms: fp32 [n_scenes, n_views, 4, 4] (img_aug @ lidar2image).  capacity >= every scene's box count, <= 4096.
+ *   endpoints: int32 [n_scenes, n_views, capacity, 8, 2], the corners' x / z, y / z (z clipped to [1e-5, 1e5]) truncated
+ *   toward zero; colors: int32 [.., capacity], the box's label; counts: int32 [n_scenes, n_views], the boxes drawn;
+ *   status: int32 [n_scenes, n_views], 0, 1 when an endpoint falls outside int32 (cv2 refuses it), 2 when the scene has
+ *   more boxes than capacity.  Slots past counts are not written.
+ * mdb_draw_box_edges_aa: for n_images = n_scenes * n_views views h x w, the 12 edges of each drawn box, in box order and
+ *   the fixed edge order, each as cv2.line(img, p0, p1, palette[colors], 1, cv2.LINE_AA) on the RGB image.  images:
+ *   uint8 [n_images, h, w, 3], or (images_is_f32) fp32 [0, 1] rounded as (x * 255).round(); out: uint8 [n_images, h, w,
+ *   3], may be a uint8 `images`.  transparent_bg: images is ignored, the boxes are drawn on black and out is uint8
+ *   [n_images, h, w, 4] with alpha 255 where any channel is non-zero.  palette: uint8 [n_colors, 3].  When any status is
+ *   non-zero nothing is written.  h, w <= 32767.
+ * ------------------------------------------------------------------------------------------------ */
+int mdb_project_boxes(const float* boxes, int box_dim, const float* sincos, const long long* labels, const int* box_offsets,
+                      int n_scenes, const float* transforms, int n_views, int capacity, int* endpoints, int* colors,
+                      int* counts, int* status, void* stream);
+int mdb_draw_box_edges_aa(const void* images, int images_is_f32, int n_images, int h, int w, const int* endpoints,
+                          const int* colors, const int* counts, const int* status, int capacity,
+                          const unsigned char* palette, int n_colors, int transparent_bg, void* out, void* stream);
+
 /* Barrier between the `world` GPUs of a sharding group over NVLink peer memory, as one stream operation (graph-capturable).
  * flag_ptrs_dev: device array of `world` pointers, entry i = GPU i's symmetric uint32[n_channels * world] flag array as mapped
  * into THIS GPU's address space; epoch_dev: this GPU's uint32[n_channels] counter; timed_out_dev: int set to 1 if a peer did
