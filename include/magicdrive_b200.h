@@ -140,6 +140,10 @@ int mdb_pool2d(const void* x, int ldx, int n, int h, int w, int c, int mode, int
                int ldo, int ho, int wo, void* stream);
 int mdb_fid_input(const void* x, int x_is_f32, int x_is_nhwc, int n, int h, int w, int quantize, int normalize, void* out,
                   int ho, int wo, void* stream);
+/* The same with f16 in place of bf16: x fp32 or f16, out f16.  The conv_in operand of an fp16 VAE's encoder
+ * (AutoencoderKL.encode); without quantize, resize or normalize each value is x rounded to f16 once. */
+int mdb_fid_input_f16(const void* x, int x_is_f32, int x_is_nhwc, int n, int h, int w, int quantize, int normalize,
+                      void* out, int ho, int wo, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * FID evaluation protocol (perception/data_prepare/val_set_gen.py:29-43, 103-116; tools/fid_score.py:361-368, 474-482):
@@ -169,6 +173,11 @@ int mdb_jpeg_roundtrip_u8(const void* x, int n, int h, int w, int quality, void*
 int mdb_conv_direct(const void* x, int x_is_f32, int n, int h, int w, int cin, const float* wgt, const float* bias,
                     int cout, int kh, int kw, int stride_h, int stride_w, int pad_h, int pad_w, int ho, int wo,
                     int silu, const void* residual, void* out, int out_is_f32, void* stream);
+/* The same with f16 in place of bf16: x f16 or fp32, out (and residual) f16 or fp32.  The decoder conv_in of an fp16 VAE
+ * (fp32 latents in, the f16 feature map out); the weights stay fp32. */
+int mdb_conv_direct_f16(const void* x, int x_is_f32, int n, int h, int w, int cin, const float* wgt, const float* bias,
+                        int cout, int kh, int kw, int stride_h, int stride_w, int pad_h, int pad_w, int ho, int wo,
+                        int silu, const void* residual, void* out, int out_is_f32, void* stream);
 
 /* GroupNorm (+SiLU) over NHWC, optionally over the channel-concat of two sources; writes one normalised tensor.
  * Replaces nn.GroupNorm + SiLU (resnet.py:535,556,598,630; transformer_2d.py:145; unet_2d_condition.py:492).
@@ -189,6 +198,9 @@ int mdb_layernorm(const void* x, long long rows, int c, int ldx, const float* ga
  * cols <= j < cols_out (K padding of the following P.V GEMM).  Used by the VAE decoder's single-head 512-wide attention
  * (unet_2d_blocks.py:433-446; attention_processor.py:1252), whose QK^T and PV products run on mdb_gemm_conv. */
 int mdb_softmax_rows(const float* s, int lds, long long rows, int cols, void* out, int ldo, int cols_out, void* stream);
+/* The same with f16 probabilities (the mid-block attention of an fp16 VAE). */
+int mdb_softmax_rows_f16(const float* s, int lds, long long rows, int cols, void* out, int ldo, int cols_out,
+                         void* stream);
 
 /* Fused multi-head attention forward, softmax(Q K^T * scale) V, bf16 in/out, fp32 softmax.
  * q: [b, Lq, heads*d] with row stride ldq; k, v: [b_kv, Lk, heads*d] with row strides ldk, ldv; out like q (ldo).

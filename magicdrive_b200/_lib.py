@@ -48,6 +48,7 @@ SIGNATURES = {
     "mdb_gemm_conv_stats_parts": (_i, [C.POINTER(GemmDesc)]),
     "mdb_gemm_conv_plan": (_i, [C.POINTER(GemmDesc), C.POINTER(C.c_int)]),
     "mdb_conv_direct": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp]),
+    "mdb_conv_direct_f16": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp]),
     "mdb_groupnorm": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp, _i, _vp, _i, _vp, _vp]),
     "mdb_groupnorm_f16": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, _i, _f, _vp, _vp, _i, _vp, _i, _vp, _vp]),
     "mdb_layernorm": (_i, [_vp, _ll, _i, _i, _vp, _vp, _f, _vp, _i, _vp]),
@@ -75,6 +76,7 @@ SIGNATURES = {
     "mdb_pack_latents_f16": (_i, [_vp, _i, _ll, _i, _i, _i, _vp, _vp]),
     "mdb_cfg_ddim_step": (_i, [_vp, _i, _i, _i, _f, _vp, _vp, _ll, _vp]),
     "mdb_softmax_rows": (_i, [_vp, _i, _ll, _i, _vp, _i, _i, _vp]),
+    "mdb_softmax_rows_f16": (_i, [_vp, _i, _ll, _i, _vp, _i, _i, _vp]),
     "mdb_pin_views": (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp, _ll, _i, _vp]),
     "mdb_peer_barrier": (_i, [_vp, _i, _i, _i, _i, _vp, _ll, _vp, _vp]),
     "mdb_prepare_boxes": (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
@@ -82,6 +84,7 @@ SIGNATURES = {
     "mdb_cfg_unipc_step": (_i, [_vp, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _ll, _vp]),
     "mdb_pool2d": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _i, _vp]),
     "mdb_fid_input": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _vp]),
+    "mdb_fid_input_f16": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _i, _vp]),
     "mdb_resample_u8": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _i,
                              _vp]),
     "mdb_jpeg_roundtrip_u8": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp]),

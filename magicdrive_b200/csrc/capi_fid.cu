@@ -2,11 +2,13 @@
 // InceptionV3 and its input step (8-bit rounding, bilinear resize to 299x299, 2x - 1).  Its convolutions run on
 // mdb_gemm_conv.  Compiled WITHOUT --use_fast_math: the resize and the averages follow ATen's fp32 arithmetic.
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <math.h>
 
 #include "../../include/magicdrive_b200.h"
 #include "common_host.h"
+#include "ptx.cuh"
 
 namespace {
 
@@ -87,6 +89,8 @@ template <>
 __device__ __forceinline__ float ldf<float>(const float* p) { return __ldg(p); }
 template <>
 __device__ __forceinline__ float ldf<__nv_bfloat16>(const __nv_bfloat16* p) { return __bfloat162float(*p); }
+template <>
+__device__ __forceinline__ float ldf<__half>(const __half* p) { return __half2float(*p); }
 
 // ATen's upsample_bilinear2d source index (align_corners=False): max(scale * (dst + 0.5) - 0.5, 0), scale = in / out
 __device__ __forceinline__ void src_index(int dst, int in, int out, int* i0, int* i1, float* l1) {
@@ -98,8 +102,8 @@ __device__ __forceinline__ void src_index(int dst, int in, int out, int* i0, int
   *l1 = real - static_cast<float>(i);
 }
 
-// one thread per output pixel: 3 channels in, 8 bf16 channels out (3..7 zero)
-template <typename T>
+// one thread per output pixel: 3 channels in, 8 bf16 channels out (3..7 zero); F16: f16 out (the encoder of an fp16 VAE)
+template <typename T, bool F16 = false>
 __global__ void fid_input_kernel(const T* __restrict__ x, int nhwc, int n, int h, int w, int quantize, int normalize,
                                  uint4* __restrict__ o, int ho, int wo) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -128,11 +132,12 @@ __global__ void fid_input_kernel(const T* __restrict__ x, int nhwc, int n, int h
     const float v = (1.f - lh) * top + lh * bot;
     res[ch] = normalize ? 2.f * v - 1.f : v;
   }
+  using A = mdb::Act<F16>;
   uint4 r;
-  __nv_bfloat162* hr = reinterpret_cast<__nv_bfloat162*>(&r);
-  hr[0] = __floats2bfloat162_rn(res[0], res[1]);
-  hr[1] = __floats2bfloat162_rn(res[2], 0.f);
-  hr[2] = __floats2bfloat162_rn(0.f, 0.f);
+  uint32_t* hr = reinterpret_cast<uint32_t*>(&r);
+  hr[0] = A::pack(res[0], res[1]);
+  hr[1] = A::pack(res[2], 0.f);
+  hr[2] = A::pack(0.f, 0.f);
   hr[3] = hr[2];
   o[i] = r;
 }
@@ -169,8 +174,12 @@ extern "C" int mdb_pool2d(const void* x, int ldx, int n, int h, int w, int c, in
   return MDB_OK;
 }
 
-extern "C" int mdb_fid_input(const void* x, int x_is_f32, int x_is_nhwc, int n, int h, int w, int quantize, int normalize,
-                             void* out, int ho, int wo, void* stream) {
+namespace {
+// x: fp32, or the element type of the output (bf16, f16 with F16)
+template <bool F16>
+int fid_input_launch(const void* x, int x_is_f32, int x_is_nhwc, int n, int h, int w, int quantize, int normalize, void* out,
+                     int ho, int wo, void* stream) {
+  using Elt = typename mdb::Act<F16>::T;
   if (!x || !out) return mdb::set_error(MDB_ERR_INVALID, "mdb_fid_input: null pointer");
   if (n <= 0 || h <= 0 || w <= 0 || ho <= 0 || wo <= 0) return mdb::set_error(MDB_ERR_INVALID, "mdb_fid_input: bad shape");
   if (reinterpret_cast<uintptr_t>(out) & 15) return mdb::set_error(MDB_ERR_INVALID, "mdb_fid_input: out must be 16-byte aligned");
@@ -178,11 +187,22 @@ extern "C" int mdb_fid_input(const void* x, int x_is_f32, int x_is_nhwc, int n, 
   const int threads = 256;
   const long long total = (long long)n * ho * wo;
   if (x_is_f32)
-    fid_input_kernel<float><<<blocks_for(total, threads), threads, 0, st>>>(static_cast<const float*>(x), x_is_nhwc, n, h, w,
-                                                                            quantize, normalize, static_cast<uint4*>(out), ho, wo);
+    fid_input_kernel<float, F16><<<blocks_for(total, threads), threads, 0, st>>>(
+        static_cast<const float*>(x), x_is_nhwc, n, h, w, quantize, normalize, static_cast<uint4*>(out), ho, wo);
   else
-    fid_input_kernel<__nv_bfloat16><<<blocks_for(total, threads), threads, 0, st>>>(
-        static_cast<const __nv_bfloat16*>(x), x_is_nhwc, n, h, w, quantize, normalize, static_cast<uint4*>(out), ho, wo);
+    fid_input_kernel<Elt, F16><<<blocks_for(total, threads), threads, 0, st>>>(
+        static_cast<const Elt*>(x), x_is_nhwc, n, h, w, quantize, normalize, static_cast<uint4*>(out), ho, wo);
   MDB_CHECK_LAUNCH("fid_input_kernel");
   return MDB_OK;
+}
+}  // namespace
+
+extern "C" int mdb_fid_input(const void* x, int x_is_f32, int x_is_nhwc, int n, int h, int w, int quantize, int normalize,
+                             void* out, int ho, int wo, void* stream) {
+  return fid_input_launch<false>(x, x_is_f32, x_is_nhwc, n, h, w, quantize, normalize, out, ho, wo, stream);
+}
+
+extern "C" int mdb_fid_input_f16(const void* x, int x_is_f32, int x_is_nhwc, int n, int h, int w, int quantize, int normalize,
+                                 void* out, int ho, int wo, void* stream) {
+  return fid_input_launch<true>(x, x_is_f32, x_is_nhwc, n, h, w, quantize, normalize, out, ho, wo, stream);
 }

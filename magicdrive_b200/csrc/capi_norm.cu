@@ -705,9 +705,12 @@ extern "C" int mdb_layernorm(const void* x, long long rows, int c, int ldx, cons
 
 // ---------------------------------------------------------------- row softmax (single-head VAE attention scores)
 namespace {
-// one warp per row: out[r, j] = exp(s[r, j] - max_r) / sum_r for j < cols, 0 for cols <= j < cols_out (bf16)
-__global__ void softmax_rows_kernel(const float* __restrict__ s, int lds, long long rows, int cols,
-                                    __nv_bfloat16* __restrict__ out, int ldo, int cols_out) {
+// one warp per row: out[r, j] = exp(s[r, j] - max_r) / sum_r for j < cols, 0 for cols <= j < cols_out (bf16, or f16 with
+// F16: an fp16 VAE)
+template <bool F16>
+__device__ __forceinline__ void softmax_rows(const float* __restrict__ s, int lds, long long rows, int cols,
+                                             typename mdb::Act<F16>::T* __restrict__ out, int ldo, int cols_out) {
+  using A = mdb::Act<F16>;
   const long long row = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
@@ -721,20 +724,43 @@ __global__ void softmax_rows_kernel(const float* __restrict__ s, int lds, long l
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
   const float inv = 1.0f / sum;
-  __nv_bfloat16* orow = out + row * ldo;
-  for (int j = lane; j < cols_out; j += 32) orow[j] = __float2bfloat16_rn(j < cols ? __expf(sr[j] - mx) * inv : 0.f);
+  typename A::T* orow = out + row * ldo;
+  for (int j = lane; j < cols_out; j += 32) orow[j] = A::from_float(j < cols ? __expf(sr[j] - mx) * inv : 0.f);
 }
-}  // namespace
+__global__ void softmax_rows_kernel(const float* __restrict__ s, int lds, long long rows, int cols,
+                                    __nv_bfloat16* __restrict__ out, int ldo, int cols_out) {
+  softmax_rows<false>(s, lds, rows, cols, out, ldo, cols_out);
+}
+__global__ void softmax_rows_f16_kernel(const float* __restrict__ s, int lds, long long rows, int cols,
+                                        __half* __restrict__ out, int ldo, int cols_out) {
+  softmax_rows<true>(s, lds, rows, cols, out, ldo, cols_out);
+}
 
-extern "C" int mdb_softmax_rows(const float* s, int lds, long long rows, int cols, void* out, int ldo, int cols_out,
-                                void* stream) {
+template <bool F16>
+int softmax_rows_launch(const float* s, int lds, long long rows, int cols, void* out, int ldo, int cols_out, void* stream) {
   if (!s || !out) return mdb::set_error(MDB_ERR_INVALID, "mdb_softmax_rows: null pointer");
   if (rows <= 0 || cols <= 0 || cols_out < cols || lds < cols || ldo < cols_out)
     return mdb::set_error(MDB_ERR_INVALID, "mdb_softmax_rows: bad shape");
   const int threads = 256;
   const long long blocks = (rows * 32 + threads - 1) / threads;
-  softmax_rows_kernel<<<static_cast<unsigned>(blocks), threads, 0, static_cast<cudaStream_t>(stream)>>>(
-      s, lds, rows, cols, static_cast<__nv_bfloat16*>(out), ldo, cols_out);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if constexpr (F16)
+    softmax_rows_f16_kernel<<<static_cast<unsigned>(blocks), threads, 0, st>>>(s, lds, rows, cols, static_cast<__half*>(out),
+                                                                               ldo, cols_out);
+  else
+    softmax_rows_kernel<<<static_cast<unsigned>(blocks), threads, 0, st>>>(s, lds, rows, cols,
+                                                                           static_cast<__nv_bfloat16*>(out), ldo, cols_out);
   MDB_CHECK_LAUNCH("softmax_rows_kernel");
   return MDB_OK;
+}
+}  // namespace
+
+extern "C" int mdb_softmax_rows(const float* s, int lds, long long rows, int cols, void* out, int ldo, int cols_out,
+                                void* stream) {
+  return softmax_rows_launch<false>(s, lds, rows, cols, out, ldo, cols_out, stream);
+}
+
+extern "C" int mdb_softmax_rows_f16(const float* s, int lds, long long rows, int cols, void* out, int ldo, int cols_out,
+                                    void* stream) {
+  return softmax_rows_launch<true>(s, lds, rows, cols, out, ldo, cols_out, stream);
 }

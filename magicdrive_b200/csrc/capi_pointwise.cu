@@ -253,8 +253,9 @@ __global__ void linear_small_f16_kernel(const float* __restrict__ in, int m, int
 
 // Direct convolution, one thread per output element (output channel fastest), fp32 accumulate.  Weights are [kh][kw][cin][cout]:
 // the threads of a warp (consecutive output channels of one pixel) read consecutive weights and broadcast-read the same input
-// value.  (With [cout][kh][kw][cin] weights every lane would walk its own row: 32 sectors per load.)
-template <typename TI>
+// value.  (With [cout][kh][kw][cin] weights every lane would walk its own row: 32 sectors per load.)  F16: a 2-byte output
+// and residual in f16 (the decoder conv_in of an fp16 VAE) in place of bf16.
+template <typename TI, bool F16 = false>
 __global__ void conv_direct_kernel(const TI* __restrict__ x, int n, int h, int w, int cin, const float* __restrict__ wgt,
                                    const float* __restrict__ bias, int cout, int kh, int kw, int sh, int sw, int ph,
                                    int pw, int ho, int wo, int silu, const void* __restrict__ residual, void* __restrict__ out,
@@ -286,8 +287,9 @@ __global__ void conv_direct_kernel(const TI* __restrict__ x, int n, int h, int w
     if (residual) acc += static_cast<const float*>(residual)[i];
     static_cast<float*>(out)[i] = acc;
   } else {
-    if (residual) acc += __bfloat162float(static_cast<const __nv_bfloat16*>(residual)[i]);
-    static_cast<__nv_bfloat16*>(out)[i] = __float2bfloat16_rn(acc);
+    using A = mdb::Act<F16>;
+    if (residual) acc += A::to_float(static_cast<const typename A::T*>(residual)[i]);
+    static_cast<typename A::T*>(out)[i] = A::from_float(acc);
   }
 }
 
@@ -511,22 +513,41 @@ extern "C" int mdb_linear_small_f16(const float* in, int m, int k, int ldi, cons
   return linear_small_launch<true>(in, m, k, ldi, w, ldw, bias, n, pre_silu, post_silu, out, ldo, stream);
 }
 
-extern "C" int mdb_conv_direct(const void* x, int x_is_f32, int n, int h, int w, int cin, const float* wgt, const float* bias,
-                               int cout, int kh, int kw, int stride_h, int stride_w, int pad_h, int pad_w, int ho, int wo,
-                               int silu, const void* residual, void* out, int out_is_f32, void* stream) {
+namespace {
+// x: fp32, or the 2-byte element type of the output (bf16, f16 with F16)
+template <bool F16>
+int conv_direct_launch(const void* x, int x_is_f32, int n, int h, int w, int cin, const float* wgt, const float* bias, int cout,
+                       int kh, int kw, int stride_h, int stride_w, int pad_h, int pad_w, int ho, int wo, int silu,
+                       const void* residual, void* out, int out_is_f32, void* stream) {
+  using Elt = typename Act<F16>::T;
   if (!x || !wgt || !out) return set_error(MDB_ERR_INVALID, "mdb_conv_direct: null pointer");
   const long long total = static_cast<long long>(n) * ho * wo * cout;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (x_is_f32)
-    conv_direct_kernel<float><<<nblocks(total, 128), 128, 0, st>>>(static_cast<const float*>(x), n, h, w, cin, wgt, bias, cout,
-                                                                   kh, kw, stride_h, stride_w, pad_h, pad_w, ho, wo, silu,
-                                                                   residual, out, out_is_f32);
+    conv_direct_kernel<float, F16><<<nblocks(total, 128), 128, 0, st>>>(static_cast<const float*>(x), n, h, w, cin, wgt, bias,
+                                                                        cout, kh, kw, stride_h, stride_w, pad_h, pad_w, ho, wo,
+                                                                        silu, residual, out, out_is_f32);
   else
-    conv_direct_kernel<__nv_bfloat16><<<nblocks(total, 128), 128, 0, st>>>(
-        static_cast<const __nv_bfloat16*>(x), n, h, w, cin, wgt, bias, cout, kh, kw, stride_h, stride_w, pad_h, pad_w, ho, wo,
-        silu, residual, out, out_is_f32);
+    conv_direct_kernel<Elt, F16><<<nblocks(total, 128), 128, 0, st>>>(static_cast<const Elt*>(x), n, h, w, cin, wgt, bias,
+                                                                      cout, kh, kw, stride_h, stride_w, pad_h, pad_w, ho, wo,
+                                                                      silu, residual, out, out_is_f32);
   MDB_CHECK_LAUNCH("conv_direct_kernel");
   return MDB_OK;
+}
+}  // namespace
+
+extern "C" int mdb_conv_direct(const void* x, int x_is_f32, int n, int h, int w, int cin, const float* wgt, const float* bias,
+                               int cout, int kh, int kw, int stride_h, int stride_w, int pad_h, int pad_w, int ho, int wo,
+                               int silu, const void* residual, void* out, int out_is_f32, void* stream) {
+  return conv_direct_launch<false>(x, x_is_f32, n, h, w, cin, wgt, bias, cout, kh, kw, stride_h, stride_w, pad_h, pad_w, ho,
+                                   wo, silu, residual, out, out_is_f32, stream);
+}
+
+extern "C" int mdb_conv_direct_f16(const void* x, int x_is_f32, int n, int h, int w, int cin, const float* wgt,
+                                   const float* bias, int cout, int kh, int kw, int stride_h, int stride_w, int pad_h, int pad_w,
+                                   int ho, int wo, int silu, const void* residual, void* out, int out_is_f32, void* stream) {
+  return conv_direct_launch<true>(x, x_is_f32, n, h, w, cin, wgt, bias, cout, kh, kw, stride_h, stride_w, pad_h, pad_w, ho,
+                                  wo, silu, residual, out, out_is_f32, stream);
 }
 
 extern "C" int mdb_pack_latents(const void* x, int x_is_f32, long long pix, int cin, int cpad, int repeat, void* out,

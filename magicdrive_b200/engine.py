@@ -17,16 +17,16 @@ from typing import Dict, List, Optional
 
 import torch
 
-from . import arch, f16_ops, ops
+from . import arch, f16_ops, ops, vae_f16_ops
 from .params import pack_conv_weight, pack_conv_weight_k64, pack_geglu
 
 BF16, F16, F32 = torch.bfloat16, torch.float16, torch.float32
 
 
 def storage_dtype(sd: Dict[str, torch.Tensor]) -> torch.dtype:
-    """Activation and weight storage of a UNet / ControlNet engine: f16 when every floating tensor of the module is fp16
-    (from_pretrained(torch_dtype=torch.float16), .to(torch.float16): the precision the reference's inference runs), bf16
-    for any other parameter dtype.  The VAE, CLIP and Inception engines are bf16 whatever their parameters."""
+    """Activation and weight storage of a UNet / ControlNet / VAE engine: f16 when every floating tensor of the module is
+    fp16 (from_pretrained(torch_dtype=torch.float16), .to(torch.float16): the precision the reference's inference runs),
+    bf16 for any other parameter dtype.  The CLIP and Inception engines are bf16 whatever their parameters."""
     fl = [v.dtype for v in sd.values() if v.is_floating_point()]
     return F16 if fl and all(d == F16 for d in fl) else BF16
 
@@ -92,14 +92,16 @@ class _Weights:
         return self.t[p + ".wk"], self.t[p + ".b"]
 
     def conv_n_padded(self, p, npad):
-        """3x3 filter with the output channels zero-padded to `npad` (conv_out: 4 -> 8, the kernel's N granularity)."""
+        """3x3 filter with the output channels zero-padded to `npad` (conv_out: 4 -> 8, the kernel's N granularity), K64-packed
+        (the plain layout when the input channels are a multiple of 64; a VAE decoder whose top block has 32 channels needs
+        the padded one)."""
         if p + ".wn" not in self.t:
             w = self.raw(p + ".weight").float()
             wp = torch.zeros((npad, *w.shape[1:]), dtype=F32, device=w.device)
             wp[: w.shape[0]] = w
             bp = torch.zeros((npad,), dtype=F32, device=w.device)
             bp[: w.shape[0]] = self.raw(p + ".bias").float()
-            self.t[p + ".wn"] = pack_conv_weight(wp, self.dtype)
+            self.t[p + ".wn"] = pack_conv_weight_k64(wp, dtype=self.dtype)
             self.t[p + ".bn"] = bp
         return self.t[p + ".wn"], self.t[p + ".bn"]
 
@@ -664,18 +666,21 @@ class _VaeEngine:
     """The blocks the VAE's encoder and decoder share, on the same operators as the denoising path (implicit-GEMM 3x3
     convolutions, single-kernel GroupNorm+SiLU).  The mid block's single-head attention is 512 wide — beyond the fused
     attention kernels' head dims — and runs as three tensor-core GEMMs per image around a row softmax:
-    S = Q K^T (fp32, scaled), P = softmax(S) (bf16, key count padded to a K block), V^T = W_v X^T, O = P V + b_v."""
+    S = Q K^T (fp32, scaled), P = softmax(S) (bf16, key count padded to a K block), V^T = W_v X^T, O = P V + b_v.
+    Activations and weight matrices are bf16, or f16 for a VAE whose parameters are all fp16 (storage_dtype; P too);
+    biases, GroupNorm affines and accumulation stay fp32."""
 
     def __init__(self, cfg: arch.VaeConfig, sd, device):
         self.cfg, self.device = cfg, device
-        self.W = _Weights(sd, device)
+        self.dtype = storage_dtype(sd)
+        self.W = _Weights(sd, device, self.dtype)
 
     def _conv(self, p):
-        """Conv2d `p` as a K64-packed bf16 matrix (the plain (tap, channel) layout when the input channels are a multiple
-        of 64, as in SD-1.5) and an fp32 bias."""
+        """Conv2d `p` as a K64-packed matrix in the storage type (the plain (tap, channel) layout when the input channels
+        are a multiple of 64, as in SD-1.5) and an fp32 bias."""
         W = self.W
         if p + ".w64" not in W.t:
-            W.t[p + ".w64"] = pack_conv_weight_k64(W.raw(p + ".weight").float())
+            W.t[p + ".w64"] = pack_conv_weight_k64(W.raw(p + ".weight").float(), dtype=W.dtype)
             W.t[p + ".b"] = _f32(W.raw(p + ".bias"))
         return W.t[p + ".w64"], W.t[p + ".b"]
 
@@ -719,6 +724,7 @@ class _VaeEngine:
                         torch.empty((x.n * L, C), dtype=q.dtype, device=dev), torch.zeros((x.n * L + lp - L, C), dtype=q.dtype, device=dev),
                         torch.zeros((x.n * L + lp - L, C), dtype=q.dtype, device=dev))
         sbuf, vtbuf, o, kbuf, tbuf = W.t[key]
+        softmax_rows = vae_f16_ops.softmax_rows_f16 if self.dtype == F16 else ops.softmax_rows
         ops.linear(t, wk, bias=bk, out=kbuf[: x.n * L], ldo=C)
         if lp != L:  # the V^T GEMM likewise takes lp token rows per image (finite values in the spare columns, P is zero there)
             tbuf[: x.n * L].copy_(t)
@@ -726,7 +732,7 @@ class _VaeEngine:
         for i in range(x.n):
             rows = slice(i * L, (i + 1) * L)
             ops.linear(q[rows], kbuf[i * L: i * L + lp], out_f32=True, out_scale=C ** -0.5, out=sbuf[i], ldo=lp)  # [L, lp]: q . k_j / sqrt(C)
-            p = ops.softmax_rows(sbuf[i], L, lp)                                                    # bf16, padded keys get 0
+            p = softmax_rows(sbuf[i], L, lp)                                                        # padded keys get 0
             ops.linear(wv, t[i * L: i * L + lp] if lp != L else t[rows], out=vtbuf[i], ldo=lp)      # [C, lp] = W_v X^T  (V^T, no bias)
             ops.linear(p, vtbuf[i], bias=bv, out=o[rows], ldo=C)                                    # P V + b_v (rows of P sum to 1)
         wo, bo = W.lin(a + ".to_out.0")
@@ -746,7 +752,9 @@ class VaeDecoderEngine(_VaeEngine):
 
     def decode(self, z_nhwc: torch.Tensor, n: int, h: int, w: int, scale: float = 1.0, to_unit_range: bool = False):
         """z_nhwc: fp32 [n*h*w, 4] latents (the denoiser's resident layout); `scale` multiplies them first
-        (1 / scaling_factor).  Returns fp32 [n, 8h, 8w, 3] (with to_unit_range: image / 2 + 0.5 clamped to [0, 1])."""
+        (1 / scaling_factor).  Returns fp32 [n, 8h, 8w, 3] (with to_unit_range: image / 2 + 0.5 clamped to [0, 1]).
+        post_quant_conv (with the scale folded into its fp32 weights) runs in fp32; conv_in reads its fp32 output and writes
+        the first feature map in the storage type."""
         cfg, W = self.cfg, self.W
         key = ("pq", float(scale))
         if key not in W.t:  # 1x1 post_quant_conv with the latent scale folded into its weights
@@ -756,7 +764,8 @@ class VaeDecoderEngine(_VaeEngine):
         x = ops.conv_direct(z_nhwc.reshape(n, h, w, lc), wq, bq, n=n, h=h, w=w, cin=lc, cout=lc, k=1, pad=(0, 0), out_f32=True)
         wd, bd = W.conv_direct("decoder.conv_in")
         c = cfg.block_out_channels[-1]
-        x = ops.conv_direct(x, wd, bd, n=n, h=h, w=w, cin=lc, cout=c, k=3)
+        conv_direct = vae_f16_ops.conv_direct_f16 if self.dtype == F16 else ops.conv_direct
+        x = conv_direct(x, wd, bd, n=n, h=h, w=w, cin=lc, cout=c, k=3)
         x = FMap(x.reshape(n * h * w, c), n, h, w, c)
         x = self._resnet("decoder.mid_block.resnets.0", x, c)
         x = self._attention("decoder.mid_block.attentions.0", x)
@@ -787,11 +796,11 @@ class VaeDecoderEngine(_VaeEngine):
 
 class VaeEncoderEngine(_VaeEngine):
     """AutoencoderKL.encode (autoencoder_kl.py:160-171 -> Encoder.forward, vae.py:108-149): camera images to the latent
-    moments, for given-view generation from real views (demo/run_cond_on_view.py:80-85).  mdb_fid_input turns the RGB
-    batch into conv_in's 8-channel bf16 operand (one partial K block per tap); each Downsample2D(padding=0), which pads
-    the bottom and right edge by one (resnet.py:199,213-217), is one stride-2 convolution with end padding 1; quant_conv
-    is folded into conv_out: W = Q W_out, b = Q b_out + b_q, composed in fp32 and rounded to bf16 once, so the moments
-    come out of one GEMM epilogue in fp32."""
+    moments, for given-view generation from real views (demo/run_cond_on_view.py:80-85).  mdb_fid_input (mdb_fid_input_f16)
+    turns the RGB batch into conv_in's 8-channel bf16 (f16) operand (one partial K block per tap); each
+    Downsample2D(padding=0), which pads the bottom and right edge by one (resnet.py:199,213-217), is one stride-2 convolution
+    with end padding 1; quant_conv is folded into conv_out: W = Q W_out, b = Q b_out + b_q, composed in fp32 and rounded to
+    the storage type once, so the moments come out of one GEMM epilogue in fp32."""
 
     def __init__(self, cfg: arch.VaeConfig, sd, device):
         super().__init__(cfg, sd, device)
@@ -805,7 +814,7 @@ class VaeEncoderEngine(_VaeEngine):
         if "encoder.conv_in.w8" not in W.t:
             w = W.raw("encoder.conv_in.weight").float()
             w = torch.cat([w, w.new_zeros((w.shape[0], 8 - w.shape[1], *w.shape[2:]))], 1)
-            W.t["encoder.conv_in.w8"] = pack_conv_weight_k64(w)
+            W.t["encoder.conv_in.w8"] = pack_conv_weight_k64(w, dtype=W.dtype)
             W.t["encoder.conv_in.b"] = _f32(W.raw("encoder.conv_in.bias"))
         return W.t["encoder.conv_in.w8"], W.t["encoder.conv_in.b"]
 
@@ -826,13 +835,16 @@ class VaeEncoderEngine(_VaeEngine):
         return W.t[key]
 
     def encode(self, x: torch.Tensor, mean_scale: float = 1.0):
-        """x: (n, 3, H, W) fp32 or bf16 images in [-1, 1] on the device.  Returns (moments, h, w): fp32
+        """x: (n, 3, H, W) fp32 or storage-type (bf16 / f16) images in [-1, 1] on the device.  Returns (moments, h, w): fp32
         [n*h*w, 2*latent_channels rounded up to 8] NHWC, mean channels first and multiplied by `mean_scale`, then logvar."""
         cfg, W = self.cfg, self.W
         n, cin, h, w = x.shape
         if cin != 3:
             raise ValueError(f"VaeEncoderEngine reads RGB images, got {cin} channels")
-        a = ops.fid_input(x, nhwc=False, quantize=False, normalize=False)  # bf16 [n*h*w, 8], channels 3..7 zero
+        if self.dtype == F16:  # [n*h*w, 8] in the storage type, channels 3..7 zero
+            a = vae_f16_ops.fid_input_f16(x, nhwc=False, quantize=False, normalize=False)
+        else:
+            a = ops.fid_input(x, nhwc=False, quantize=False, normalize=False)
         wi, bi = self._conv_in()
         c = cfg.block_out_channels[0]
         x = FMap(ops.gemm_conv(a, wi, n_img=n, h_in=h, w_in=w, c0=8, lda0=8, n_out=c, taps=3, pad=1, bias=bi), n, h, w, c)

@@ -526,7 +526,9 @@ class AutoencoderKL(_B200Module):
     The decoder (`decoder.*`, `post_quant_conv.*`) is always present.  The encoder (`encoder.*`, `quant_conv.*`) is kept
     when a state dict holds its complete set for this config; a decoder-only state dict, or one with only part of the
     encoder, loads the decoder alone (the encoder keys are ignored) and `encode` raises NotImplementedError naming what is
-    missing."""
+    missing.
+    A VAE whose floating parameters are all fp16 (from_pretrained(torch_dtype=torch.float16), .to(torch.float16)) decodes
+    and encodes in f16, any other in bf16 (engine.storage_dtype); `.to()` rebuilds both engines and drops their graphs."""
 
     def __init__(self, **kwargs):
         super().__init__()
@@ -595,11 +597,11 @@ class AutoencoderKL(_B200Module):
 
     @torch.no_grad()
     def encode(self, x: torch.Tensor, return_dict: bool = True):
-        """x: (n, 3, H, W) images in [-1, 1] on the device, any float dtype (fp32 and bf16 are read directly) ->
-        AutoencoderKLOutput(latent_dist=DiagonalGaussianDistribution) over (n, 2 * latent_channels, h, w) moments in x's
-        dtype, h = H / 8 for the SD-1.5 layout (autoencoder_kl.py:160-171)."""
+        """x: (n, 3, H, W) images in [-1, 1] on the device, any float dtype (fp32 and the engine's storage type, bf16 or f16
+        for an fp16 VAE, are read directly) -> AutoencoderKLOutput(latent_dist=DiagonalGaussianDistribution) over
+        (n, 2 * latent_channels, h, w) moments in x's dtype, h = H / 8 for the SD-1.5 layout (autoencoder_kl.py:160-171)."""
         eng = self.encoder_engine()
-        xin = x if x.dtype in (F32, BF16) else x.float()
+        xin = x if x.dtype in (F32, eng.dtype) else x.float()
         m, h, w = eng.encode(xin.to(self.device).contiguous())
         moments = m.view(x.shape[0], h, w, -1)[..., : eng.moments].permute(0, 3, 1, 2).to(x.dtype)
         dist = DiagonalGaussianDistribution(moments)
@@ -613,7 +615,7 @@ class AutoencoderKL(_B200Module):
         b, n_cam = pixel_values.shape[:2]
         eng = self.encoder_engine()
         x = pixel_values.to(self.device).reshape(b * n_cam, *pixel_values.shape[2:])
-        x = (x if x.dtype in (F32, BF16) else x.float()).contiguous()
+        x = (x if x.dtype in (F32, eng.dtype) else x.float()).contiguous()
         lc, sf = self.arch_cfg.latent_channels, float(self.config["scaling_factor"])
         run = lambda xx: eng.encode(xx, mean_scale=sf)
         if not (self.use_cuda_graph and x.is_cuda):
@@ -640,7 +642,8 @@ class AutoencoderKL(_B200Module):
 
     @torch.no_grad()
     def decode(self, z: torch.Tensor, return_dict: bool = True):
-        """z: (n, 4, h, w) latents already divided by scaling_factor, as the pipeline passes them -> (n, 3, 8h, 8w)."""
+        """z: (n, 4, h, w) latents already divided by scaling_factor, as the pipeline passes them (any float dtype; an fp16
+        VAE's decoder reads them in fp32 and computes in f16) -> (n, 3, 8h, 8w) in z's dtype."""
         n, c, h, w = z.shape
         z_nhwc = z.to(F32).permute(0, 2, 3, 1).contiguous().view(-1, c)
         img = self.engine().decode(z_nhwc, n, h, w).permute(0, 3, 1, 2).to(z.dtype)
