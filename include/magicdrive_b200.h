@@ -166,6 +166,25 @@ int mdb_resample_u8(const void* x, int x_is_f32, int x_is_nhwc, int n, int h, in
                     void* tmp, void* out, int out_h, int out_w, int top, int left, void* stream);
 int mdb_jpeg_roundtrip_u8(const void* x, int n, int h, int w, int quality, void* planes, void* out, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * JPEG files of generated views (perception/data_prepare/val_set_gen.py:29-43, copy_save_image's PIL save).
+ * mdb_jpeg_encode_u8: uint8 NHWC RGB [n, h, w, 3] (n in 1..65535, h and w in 1..65535) -> the files
+ *   PIL.Image.fromarray(x[i]).save(f, "JPEG", quality=quality) writes, byte for byte: baseline, 4:2:0, the standard
+ *   quantisation tables scaled as in mdb_jpeg_roundtrip_u8 and the standard Huffman tables, no restart interval.  Each
+ *   file is the MDB_JPEG_HEADER_BYTES-byte header, the entropy-coded data and EOI.  The files are written back to back in
+ *   `out` (out_bytes bytes).  meta: 8-byte aligned device int64 [n, 3], per image (entropy-coded bytes before stuffing,
+ *   file length, offset of the file in out); the length is -1 when the scratch was too small to count it, the offset -1
+ *   when the files were not written (scratch or out too small: nothing is written to out then, and meta says what is
+ *   needed).  scratch: 256-byte aligned, scratch_bytes >= mdb_jpeg_scratch_bytes(n, h, w, chunks) for `chunks` 4 KiB
+ *   chunks of entropy-coded data, each image taking ceil(entropy-coded bytes / 4096) of them (at least n are required).
+ *   Arguments are checked before any launch; the lengths are known only on the device, so the caller reads meta.
+ * mdb_jpeg_scratch_bytes: that scratch size, or -1 for bad arguments.
+ * ------------------------------------------------------------------------------------------------ */
+#define MDB_JPEG_HEADER_BYTES 623
+long long mdb_jpeg_scratch_bytes(int n, int h, int w, long long chunks);
+int mdb_jpeg_encode_u8(const void* x, int n, int h, int w, int quality, void* scratch, long long scratch_bytes, void* out,
+                       long long out_bytes, long long* meta, void* stream);
+
 /* Direct (CUDA-core) convolution for tiny channel counts: conv_in 4->320 (unet_2d_condition.py:231),
  * conv_out 320->4 (:503), BEV map encoder (magicdrive/networks/map_embedder.py:66-76).
  * x: [n, h, w, cin] bf16 or fp32; w: fp32 [kh, kw, cin, cout] (output channel innermost: coalesced across a warp);

@@ -88,6 +88,8 @@ SIGNATURES = {
     "mdb_resample_u8": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _i, _i,
                              _vp]),
     "mdb_jpeg_roundtrip_u8": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "mdb_jpeg_scratch_bytes": (_ll, [_i, _i, _i, _ll]),
+    "mdb_jpeg_encode_u8": (_i, [_vp, _i, _i, _i, _i, _vp, _ll, _vp, _ll, _vp, _vp]),
     "mdb_project_boxes": (_i, [_vp, _i, _vp, _vp, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "mdb_draw_box_edges_aa": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _vp, _vp]),
 }

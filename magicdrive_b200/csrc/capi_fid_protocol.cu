@@ -8,6 +8,7 @@
 
 #include "../../include/magicdrive_b200.h"
 #include "common_host.h"
+#include "jpeg_fdct.cuh"
 
 namespace {
 
@@ -129,44 +130,6 @@ int launch_resample(Src src, int n, const int* coef_w, int taps_w, const int* co
 }
 
 // ----------------------------------------------------------------------------------------------------------------- JPEG
-// Integer Loeffler-Ligtenberg-Moschytz 8-point DCT pair: 13 fraction bits in the rotations, 2 extra bits kept between
-// the passes.  The forward output is 8x the orthonormal DCT; the inverse output carries 3 more bits that its second pass
-// removes.
-constexpr int kConstBits = 13, kPass1Bits = 2;
-constexpr int F0298 = 2446, F0390 = 3196, F0541 = 4433, F0765 = 6270, F0899 = 7373, F1175 = 9633;
-constexpr int F1501 = 12299, F1847 = 15137, F1961 = 16069, F2053 = 16819, F2562 = 20995, F3072 = 25172;
-
-__device__ __forceinline__ int descale(int x, int n) { return (x + (1 << (n - 1))) >> n; }
-
-// forward transform of 8 values at p[0], p[s], ..., p[7 s]; the first pass keeps the even outputs exact (shifted left),
-// the second rounds them away
-template <bool kFirst>
-__device__ __forceinline__ void fdct8(int* p, int s) {
-  constexpr int odd = kFirst ? kConstBits - kPass1Bits : kConstBits + kPass1Bits;
-  const int t0 = p[0] + p[7 * s], t7 = p[0] - p[7 * s];
-  const int t1 = p[s] + p[6 * s], t6 = p[s] - p[6 * s];
-  const int t2 = p[2 * s] + p[5 * s], t5 = p[2 * s] - p[5 * s];
-  const int t3 = p[3 * s] + p[4 * s], t4 = p[3 * s] - p[4 * s];
-  const int t10 = t0 + t3, t13 = t0 - t3, t11 = t1 + t2, t12 = t1 - t2;
-  if (kFirst) {
-    p[0] = (t10 + t11) * (1 << kPass1Bits);
-    p[4 * s] = (t10 - t11) * (1 << kPass1Bits);
-  } else {
-    p[0] = descale(t10 + t11, kPass1Bits);
-    p[4 * s] = descale(t10 - t11, kPass1Bits);
-  }
-  const int e = (t12 + t13) * F0541;
-  p[2 * s] = descale(e + t13 * F0765, odd);
-  p[6 * s] = descale(e - t12 * F1847, odd);
-  const int z5 = (t4 + t6 + t5 + t7) * F1175;
-  const int z1 = -(t4 + t7) * F0899, z2 = -(t5 + t6) * F2562;
-  const int z3 = -(t4 + t6) * F1961 + z5, z4 = -(t5 + t7) * F0390 + z5;
-  p[7 * s] = descale(t4 * F0298 + z1 + z3, odd);
-  p[5 * s] = descale(t5 * F2053 + z2 + z4, odd);
-  p[3 * s] = descale(t6 * F3072 + z2 + z3, odd);
-  p[s] = descale(t7 * F1501 + z1 + z4, odd);
-}
-
 template <int kShift>
 __device__ __forceinline__ void idct8(int* p, int s) {
   const int e = (p[2 * s] + p[6 * s]) * F0541;
@@ -196,19 +159,6 @@ __device__ __forceinline__ uint8_t range_limit(int x) {
   return static_cast<uint8_t>(x < 0 ? 0 : (x > 255 ? 255 : x));
 }
 
-// BT.601 RGB -> YCbCr in 16 fraction bits; Cb and Cr round with 1/2 - 2^-16 so that they never exceed 255
-constexpr int kRY = 19595, kGY = 38470, kBY = 7471, kRCb = 11059, kGCb = 21709, kHalf = 32768;  // FIX(0.299) ...
-constexpr int kGCr = 27439, kBCr = 5329, kHalfC = 32768;                                         // FIX(0.41869) ...
-__device__ __forceinline__ void rgb_ycc(int r, int g, int b, int* y, int* cb, int* cr) {
-  *y = (kRY * r + kGY * g + kBY * b + kHalf) >> 16;
-  *cb = (-kRCb * r - kGCb * g + kHalfC * b + (128 << 16) + kHalf - 1) >> 16;
-  *cr = (kHalfC * r - kGCr * g - kBCr * b + (128 << 16) + kHalf - 1) >> 16;
-}
-
-struct QuantTables {
-  int q[2][64];  // luma, chroma; natural order
-};
-
 // One CTA per 16 x 16 MCU of one image: colour conversion, chroma averaging, and for each of the six 8 x 8 blocks the
 // forward DCT, quantisation, dequantisation and inverse DCT.  Writes the decoder's reconstructed planes: Y [hp, wp] and
 // Cb, Cr [hp / 2, wp / 2] per image (hp, wp: h, w rounded up to 16).
@@ -218,36 +168,8 @@ __global__ void __launch_bounds__(256) jpeg_code_mcu_kernel(const uint8_t* __res
   const int mcus_x = (w + 15) >> 4;
   const int my = blockIdx.x / mcus_x, mx = blockIdx.x % mcus_x, img = blockIdx.y;
   const int hp = ((h + 15) >> 4) << 4, wp = ((w + 15) >> 4) << 4;
-  const int hc = (h + 1) >> 1;
-  const uint8_t* src = x + static_cast<long long>(img) * h * w * 3;
   const int t = threadIdx.x;
-  auto pixel = [&](int yy, int xx, int* r, int* g, int* b) {
-    const uint8_t* p = src + (static_cast<long long>(yy) * w + xx) * 3;
-    *r = p[0], *g = p[1], *b = p[2];
-  };
-  {  // luma: the last row and column replicated
-    const int py = t >> 4, px = t & 15;
-    int r, g, b, y, cb, cr;
-    pixel(min(my * 16 + py, h - 1), min(mx * 16 + px, w - 1), &r, &g, &b);
-    rgb_ycc(r, g, b, &y, &cb, &cr);
-    blk[(py >> 3) * 2 + (px >> 3)][(py & 7) * 8 + (px & 7)] = y - 128;
-  }
-  if (t < 64) {  // chroma: 2 x 2 sums of full-resolution samples (columns replicated, rows replicated to an even count),
-                 // bias 1, 2, 1, 2 along the row; chroma rows past the image replicate the last chroma row
-    const int cy = t >> 3, cx = t & 7;
-    const int gy = min(my * 8 + cy, hc - 1), gx = mx * 8 + cx;
-    int scb = 0, scr = 0;
-#pragma unroll
-    for (int d = 0; d < 4; ++d) {
-      int r, g, b, y, cb, cr;
-      pixel(min(2 * gy + (d >> 1), h - 1), min(2 * gx + (d & 1), w - 1), &r, &g, &b);
-      rgb_ycc(r, g, b, &y, &cb, &cr);
-      scb += cb, scr += cr;
-    }
-    const int bias = (gx & 1) ? 2 : 1;
-    blk[4][t] = ((scb + bias) >> 2) - 128;
-    blk[5][t] = ((scr + bias) >> 2) - 128;
-  }
+  load_mcu(x, h, w, img, my, mx, blk);
   __syncthreads();
   const int b = t >> 3, k = t & 7;  // 48 threads: block b, row / column k
   if (t < 48) fdct8<true>(&blk[b][k * 8], 1);
@@ -328,16 +250,6 @@ __global__ void jpeg_color_kernel(const uint8_t* __restrict__ planes, int n, int
   o[2] = clamp255(y + ((kCbB * cb + kHalf) >> 16));
 }
 
-// ITU-T T.81 Annex K.1, natural order
-constexpr unsigned char kStdLuma[64] = {16, 11, 10, 16, 24,  40,  51,  61,  12, 12, 14, 19, 26,  58,  60,  55,
-                                        14, 13, 16, 24, 40,  57,  69,  56,  14, 17, 22, 29, 51,  87,  80,  62,
-                                        18, 22, 37, 56, 68,  109, 103, 77,  24, 35, 55, 64, 81,  104, 113, 92,
-                                        49, 64, 78, 87, 103, 121, 120, 101, 72, 92, 95, 98, 112, 100, 103, 99};
-constexpr unsigned char kStdChroma[64] = {17, 18, 24, 47, 99, 99, 99, 99, 18, 21, 26, 66, 99, 99, 99, 99,
-                                          24, 26, 56, 99, 99, 99, 99, 99, 47, 66, 99, 99, 99, 99, 99, 99,
-                                          99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99,
-                                          99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99};
-
 }  // namespace
 
 extern "C" int mdb_resample_u8(const void* x, int x_is_f32, int x_is_nhwc, int n, int h, int w, const int* coef_w,
@@ -380,13 +292,7 @@ extern "C" int mdb_jpeg_roundtrip_u8(const void* x, int n, int h, int w, int qua
     return mdb::set_error(MDB_ERR_INVALID, "mdb_jpeg_roundtrip_u8: planes must be 8-byte aligned");
   if (static_cast<long long>((h + 15) / 16) * ((w + 15) / 16) > 0x7fffffffLL || n > 65535)
     return mdb::set_error(MDB_ERR_UNSUPPORTED, "mdb_jpeg_roundtrip_u8: too many MCUs or images");
-  QuantTables qt;
-  const int scale = quality < 50 ? 5000 / quality : 200 - 2 * quality;
-  for (int i = 0; i < 64; ++i) {
-    const int l = (kStdLuma[i] * scale + 50) / 100, c = (kStdChroma[i] * scale + 50) / 100;
-    qt.q[0][i] = l < 1 ? 1 : (l > 255 ? 255 : l);
-    qt.q[1][i] = c < 1 ? 1 : (c > 255 ? 255 : c);
-  }
+  const QuantTables qt = quant_tables(quality);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const dim3 grid(((h + 15) / 16) * ((w + 15) / 16), n);
   jpeg_code_mcu_kernel<<<grid, 256, 0, st>>>(static_cast<const uint8_t*>(x), h, w, qt, static_cast<uint8_t*>(planes));

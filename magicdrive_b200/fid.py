@@ -8,6 +8,7 @@ so a generated set's FID needs no PNGs on disk.  `FIDProtocol` instead reproduce
 through it compare with the published FIDs.  Nothing here downloads weights: pass a model, or the path of the
 pytorch-fid weights file.
 """
+import copy
 import os
 import pathlib
 
@@ -15,7 +16,7 @@ import numpy as np
 import torch
 from scipy import linalg
 
-from . import image_ops
+from . import image_ops, jpeg_ops
 from .models import InceptionV3
 
 IMAGE_EXTENSIONS = {"bmp", "jpg", "jpeg", "pgm", "png", "ppm", "tif", "tiff", "webp"}
@@ -250,10 +251,9 @@ class FIDProtocol:
         graph.replay()
         return out.clone()
 
-    @torch.no_grad()
-    def generated(self, images: torch.Tensor) -> torch.Tensor:
-        """Device views in [0, 1], (S, n_cam, H, W, 3) or (N, 3, H, W), fp32 or bf16 (or uint8 (N, H, W, 3) already
-        rounded) -> uint8 (N, h, w, 3): what the reference scores for them."""
+    @staticmethod
+    def _views(images):
+        """(views [N, ...] contiguous, uint8 or fp32, nhwc) of generated()'s accepted inputs."""
         if images.dim() == 5 and images.shape[-1] == 3:
             x, nhwc = images.reshape(-1, *images.shape[2:]), True
         elif images.dim() == 4 and images.dtype == torch.uint8 and images.shape[-1] == 3:
@@ -264,7 +264,24 @@ class FIDProtocol:
             raise ValueError(f"expected (S, n_cam, H, W, 3) or (N, 3, H, W) images, got {tuple(images.shape)}")
         if x.dtype != torch.uint8:
             x = x.float()
-        return self._run("generated", self._generated, x.contiguous(), nhwc)
+        return x.contiguous(), nhwc
+
+    @torch.no_grad()
+    def generated(self, images: torch.Tensor) -> torch.Tensor:
+        """Device views in [0, 1], (S, n_cam, H, W, 3) or (N, 3, H, W), fp32 or bf16 (or uint8 (N, H, W, 3) already
+        rounded) -> uint8 (N, h, w, 3): what the reference scores for them."""
+        x, nhwc = self._views(images)
+        return self._run("generated", self._generated, x, nhwc)
+
+    @torch.no_grad()
+    def encode_generated(self, images: torch.Tensor) -> list:
+        """The inputs of generated() -> the bytes of the `.jpg` files copy_save_image writes for them (val_set_gen.py:
+        numpy_to_pil, Resize(back_resize, BICUBIC), Pad(back_pad), PIL save at `quality`), one per view in order.  The
+        resize, pad and encoder run on the device; only the files' bytes come back."""
+        x, nhwc = self._views(images)
+        left, top, _, _ = self.back_pad
+        canvas = self._resize(x, nhwc, self.back_resize, canvas=self.canvas, offset=(top, left))
+        return jpeg_ops.encode_jpeg(canvas, self.quality)
 
     @torch.no_grad()
     def real(self, u8_images: torch.Tensor, device=None) -> torch.Tensor:
@@ -277,6 +294,45 @@ class FIDProtocol:
             device = u8_images.device if u8_images.is_cuda else torch.device("cuda")
         x = u8_images.to(device).contiguous()
         return self._run("real", lambda v: self._real(v), x, True)
+
+
+@torch.no_grad()
+def save_generated_views(images: torch.Tensor, templates, img_gen_dir, view_order, protocol: FIDProtocol = None) -> list:
+    """The reference's copy_save_image (perception/data_prepare/val_set_gen.py:29-43) for views on the device.
+
+    images: (B, T, n_cam, H, W, 3) in [0, 1] (fp32 or bf16) or uint8, generation t of batch item b; templates: B label
+    entries as the reference builds them ({"filename": n_cam camera file names, "token": ...}); view_order: the n_cam
+    camera names.  Writes <img_gen_dir>/<view>/<stem>_gen_<t>.jpg for every view, in the reference's order, and returns
+    its list: one deep copy of the template per (b, t).  protocol: the FIDProtocol whose back_resize, back_pad and
+    quality make post_trans; None is `fid.raw_output: true`, the views saved at their own size at Pillow's default
+    quality.  The directories <img_gen_dir>/<view> must exist, as the reference creates them before its loop."""
+    if images.dim() != 6 or images.shape[-1] != 3:
+        raise ValueError(f"expected (B, T, n_cam, H, W, 3) images, got {tuple(images.shape)}")
+    B, T, n_cam = images.shape[:3]
+    if len(templates) != B or len(view_order) != n_cam:
+        raise ValueError(f"{len(templates)} templates and {len(view_order)} views for images {tuple(images.shape)}")
+    for template in templates:
+        for name in template["filename"]:
+            if os.path.splitext(name)[1].lower() not in (".jpg", ".jpeg"):
+                raise ValueError(f"{name}: the views are saved as JPEG files, which need a .jpg or .jpeg name")
+    views = images.reshape(B * T, n_cam, *images.shape[3:])
+    if protocol is not None:
+        files = protocol.encode_generated(views)
+    else:
+        x = views.reshape(-1, *images.shape[3:])
+        if x.dtype != torch.uint8:  # numpy_to_pil's rounding; the resample with no size change is a copy
+            x = image_ops.resample_u8(x.float().contiguous(), x.shape[1:3], None, None)
+        files = jpeg_ops.encode_jpeg(x.contiguous())
+    tmp_all, k = [], 0
+    for template in templates:
+        for gen_id in range(T):
+            for idx, view in enumerate(view_order):
+                stem, ext = os.path.splitext(os.path.basename(template["filename"][idx]))
+                with open(os.path.join(img_gen_dir, view, f"{stem}_gen_{gen_id}{ext}"), "wb") as f:
+                    f.write(files[k])
+                k += 1
+            tmp_all.append(copy.deepcopy(template))
+    return tmp_all
 
 
 def _decode_rgb(path) -> np.ndarray:
