@@ -10,7 +10,9 @@ rejects the argument combinations the library rejects.  The pure-Python wrappers
 route of `attention` to `attention_multi`) are not restated: the real ones run over these operators.
 
 Arithmetic is fp32 from the (bf16-rounded) packed weights; activations are NOT rounded to bf16 (`ROUND_ACTIVATIONS`
-switches that on), so a host-logic mistake shows up at 1e-5, not inside bf16 noise."""
+switches that on), so a host-logic mistake shows up at 1e-5, not inside bf16 noise.  `compute(torch.float64)` switches the
+arithmetic to float64 (tests/launch_census.py takes its GEMM references from gemm_conv that way, on the operands' device)."""
+import contextlib
 import math
 
 import torch
@@ -19,11 +21,27 @@ import torch.nn.functional as F
 from magicdrive_b200 import ops
 
 ROUND_ACTIVATIONS = False
+COMPUTE = torch.float32  # the type every restatement computes in
+
+
+@contextlib.contextmanager
+def compute(dtype):
+    """Run the enclosed restatements in `dtype` arithmetic (float64: a reference for the kernels)."""
+    global COMPUTE
+    old, COMPUTE = COMPUTE, dtype
+    try:
+        yield
+    finally:
+        COMPUTE = old
+
+
+def _f(x):
+    return x.to(COMPUTE)
 
 
 def _act(x):
     """Output of a device operator: a fresh contiguous buffer (optionally with the device's bf16 rounding)."""
-    return (x.to(torch.bfloat16).float() if ROUND_ACTIVATIONS else x.float()).contiguous()
+    return _f(x.to(torch.bfloat16) if ROUND_ACTIVATIONS else x).contiguous()
 
 
 def _write(out, res, ld=None):
@@ -40,7 +58,7 @@ def _k64_filter(w, n_out, kh, kw, c0, c1):
     rounded up to 64, source 1 from column 64*ceil(c0/64)); the gaps must hold zeros."""
     p0, p1 = -(-c0 // 64) * 64, -(-c1 // 64) * 64
     assert w.shape == (n_out, kh * kw * (p0 + p1)), (tuple(w.shape), n_out, kh, kw, c0, c1)
-    wt = w.float().reshape(n_out, kh, kw, p0 + p1)
+    wt = w.to(COMPUTE).reshape(n_out, kh, kw, p0 + p1)
     assert not wt[..., c0:p0].any() and not wt[..., p0 + c1:].any(), "the K64 gaps must hold zeros"
     return torch.cat([wt[..., :c0], wt[..., p0:p0 + c1]], -1).permute(0, 3, 1, 2)
 
@@ -74,10 +92,10 @@ def gemm_conv(a0, w, *, n_img, h_in, w_in, c0, lda0, n_out, taps=1, stride=1, pa
         w_out = (w_in + 2 * pw + pad_w_end - kw) // stride + 1
     pix_in = n_img * h_in * w_in
     assert a0.shape[0] == pix_in and a0.stride(0) == lda0, (a0.shape, a0.stride(), lda0)
-    x = a0[:, :c0].float()
+    x = a0[:, :c0].to(COMPUTE)
     if c1:
         assert a1.shape[0] == pix_in and a1.stride(0) == lda1, (a1.shape, a1.stride(), lda1)
-        x = torch.cat([x, a1[:, :c1].float()], 1)
+        x = torch.cat([x, a1[:, :c1].to(COMPUTE)], 1)
     cin = c0 + c1
     x = x.reshape(n_img, h_in, w_in, cin).permute(0, 3, 1, 2)
     if pad_h_end or pad_w_end:
@@ -87,14 +105,14 @@ def gemm_conv(a0, w, *, n_img, h_in, w_in, c0, lda0, n_out, taps=1, stride=1, pa
     acc = acc.permute(0, 2, 3, 1).reshape(n_img * h_out * w_out, n_out)
     if ln is not None:  # folded LayerNorm: rstd * (acc - mean * colsum) with the producer's row statistics
         assert ln.data.shape[0] == acc.shape[0]
-        tot = ln.data.float().sum(1)
+        tot = ln.data.to(COMPUTE).sum(1)
         mean = tot[:, 0:1] / cin
         var = (tot[:, 1:2] / cin - mean * mean).clamp_min(0)
-        acc = torch.rsqrt(var + ln_eps) * (acc - mean * ln_colsum.float()[None, :])
+        acc = torch.rsqrt(var + ln_eps) * (acc - mean * ln_colsum.to(COMPUTE)[None, :])
     if bias is not None:
-        acc = acc + bias.float()
+        acc = acc + bias.to(COMPUTE)
     if rowbias is not None:
-        rb = rowbias.float()
+        rb = rowbias.to(COMPUTE)
         rb = rb.expand(n_img, -1) if rb.shape[0] == 1 else rb
         assert rb.shape[0] == n_img, (rowbias.shape, n_img)
         acc = acc + rb[:, :n_out].repeat_interleave(h_out * w_out, 0)
@@ -111,7 +129,7 @@ def gemm_conv(a0, w, *, n_img, h_in, w_in, c0, lda0, n_out, taps=1, stride=1, pa
     if residual is not None:
         r2 = residual.reshape(-1, residual.shape[-1])  # the device reads it as [pixels, ldr] through a raw pointer
         assert r2.shape[0] == res.shape[0] and r2.stride(0) == ldr, (residual.shape, ldr)
-        res = res + r2[:, :res.shape[1]].float()
+        res = res + r2[:, :res.shape[1]].to(COMPUTE)
     res = res.contiguous() if out_f32 else _act(res)
     assert out is None or (out.stride(0) if ldo is None else ldo) % 8 == 0, ldo
     res_out = _write(out, res, ldo)
@@ -128,42 +146,42 @@ def gemm_conv(a0, w, *, n_img, h_in, w_in, c0, lda0, n_out, taps=1, stride=1, pa
 def conv_direct(x, wgt, bias, *, n, h, w, cin, cout, k, stride=(1, 1), pad=(1, 1), silu=False, residual=None,
                 out_f32=False):
     assert wgt.shape == (k, k, cin, cout)
-    y = F.conv2d(x.float().reshape(n, h, w, cin).permute(0, 3, 1, 2), wgt.float().permute(3, 2, 0, 1), bias.float(),
+    y = F.conv2d(x.to(COMPUTE).reshape(n, h, w, cin).permute(0, 3, 1, 2), wgt.to(COMPUTE).permute(3, 2, 0, 1), bias.to(COMPUTE),
                  stride=stride, padding=pad)
     if silu:
         y = F.silu(y)
     y = y.permute(0, 2, 3, 1)
     if residual is not None:
-        y = y + residual.float().reshape(y.shape)
+        y = y + residual.to(COMPUTE).reshape(y.shape)
     return (y if out_f32 else _act(y)).contiguous()
 
 
 def groupnorm(x0, c0, ld0, n_img, hw, gamma, beta, eps, silu, x1=None, c1=0, ld1=0, groups=32):
     assert x0.stride(0) == ld0
-    x = x0[:, :c0].float()
+    x = x0[:, :c0].to(COMPUTE)
     if c1:
         assert x1.stride(0) == ld1
-        x = torch.cat([x, x1[:, :c1].float()], 1)
+        x = torch.cat([x, x1[:, :c1].to(COMPUTE)], 1)
     c = c0 + c1
-    y = F.group_norm(x.reshape(n_img, hw, c).permute(0, 2, 1), groups, gamma.float(), beta.float(), eps)
+    y = F.group_norm(x.reshape(n_img, hw, c).permute(0, 2, 1), groups, gamma.to(COMPUTE), beta.to(COMPUTE), eps)
     if silu:
         y = F.silu(y)
     return _act(y.permute(0, 2, 1).reshape(n_img * hw, c))
 
 
 def layernorm(x, gamma, beta, eps=1e-5):
-    return _act(F.layer_norm(x.float(), (x.shape[1],), gamma.float(), beta.float(), eps))
+    return _act(F.layer_norm(x.to(COMPUTE), (x.shape[1],), gamma.to(COMPUTE), beta.to(COMPUTE), eps))
 
 
 def softmax_rows(s, cols, cols_out):
-    p = torch.softmax(s[:, :cols].float(), -1)
+    p = torch.softmax(s[:, :cols].to(COMPUTE), -1)
     return _act(F.pad(p, (0, cols_out - cols)))
 
 
 def _heads(t, ld, batches, length, heads, d):
     """[batches * length, >= heads * d] rows with stride ld -> [batches, heads, length, d]."""
     assert t.stride(0) == ld, (t.stride(), ld)
-    return t[:, :heads * d].float().reshape(batches, length, heads, d).transpose(1, 2)
+    return t[:, :heads * d].to(COMPUTE).reshape(batches, length, heads, d).transpose(1, 2)
 
 
 def attention_multi(q, sources, *, b, heads, lq, lk, d, ldq, scale, kv_index, n_sets=1, out=None, kv_len=None):
@@ -218,14 +236,14 @@ def clip_embed(ids, tok, pos, out=None):
     n_seq, ln = ids.shape
     assert ids.dtype in (torch.int32, torch.int64) and pos.shape[0] >= ln
     bad = (ids < 0) | (ids >= tok.shape[0])
-    x = tok.float()[ids.clamp(0, tok.shape[0] - 1).long()] + pos.float()[:ln][None]
+    x = tok.to(COMPUTE)[ids.clamp(0, tok.shape[0] - 1).long()] + pos.to(COMPUTE)[:ln][None]
     x = _act(torch.where(bad[..., None], torch.full_like(x, math.nan), x).reshape(n_seq * ln, -1))
     stats = torch.stack([x.sum(1), (x * x).sum(1)], -1)[:, None]
     return _write(out, x), ops.RowStats(stats.contiguous(), 1)
 
 
 def add(a, b):
-    return _act(a.float() + b.float())
+    return _act(a.to(COMPUTE) + b.to(COMPUTE))
 
 
 def nearest_index(n_in, n_out):
@@ -236,19 +254,19 @@ def nearest_index(n_in, n_out):
 
 
 def upsample_nearest(x, n, h, w, c, ho, wo):
-    xi = x.float().reshape(n, h, w, c)
+    xi = x.to(COMPUTE).reshape(n, h, w, c)
     return xi[:, nearest_index(h, ho)][:, :, nearest_index(w, wo)].reshape(n * ho * wo, c).contiguous()
 
 
 def adaptive_avgpool(x, n, h, w, c, ho, wo, silu=False):
-    y = F.adaptive_avg_pool2d(x.float().reshape(n, h, w, c).permute(0, 3, 1, 2), (ho, wo))
+    y = F.adaptive_avg_pool2d(x.to(COMPUTE).reshape(n, h, w, c).permute(0, 3, 1, 2), (ho, wo))
     y = F.silu(y) if silu else y
     return y.permute(0, 2, 3, 1).contiguous()
 
 
 def pool2d(x, *, n, h, w, c, mode, k=3, stride=1, pad=0, ldx=None, out=None, ldo=None):
     assert x.stride(0) == (c if ldx is None else ldx)
-    xi = x[:, :c].float().reshape(n, h, w, c).permute(0, 3, 1, 2)
+    xi = x[:, :c].to(COMPUTE).reshape(n, h, w, c).permute(0, 3, 1, 2)
     if mode == ops.POOL_GLOBAL_AVG:  # fp32 output
         return _write(out, xi.mean((2, 3)), ldo)
     assert mode in (ops.POOL_MAX, ops.POOL_AVG), mode
@@ -258,7 +276,7 @@ def pool2d(x, *, n, h, w, c, mode, k=3, stride=1, pad=0, ldx=None, out=None, ldo
 
 
 def fid_input(x, *, nhwc, quantize, normalize, size=None):
-    x = (x.permute(0, 3, 1, 2) if nhwc else x).float()
+    x = (x.permute(0, 3, 1, 2) if nhwc else x).to(COMPUTE)
     assert x.shape[1] == 3
     if quantize:
         x = torch.round(x * 255).clamp(0, 255) / 255
@@ -270,35 +288,35 @@ def fid_input(x, *, nhwc, quantize, normalize, size=None):
 
 
 def linear_small(x, w, bias=None, pre_silu=False, post_silu=False):
-    h = F.silu(x.float()) if pre_silu else x.float()
-    y = h @ w.float().t()
+    h = F.silu(x.to(COMPUTE)) if pre_silu else x.to(COMPUTE)
+    y = h @ w.to(COMPUTE).t()
     if bias is not None:
-        y = y + bias.float()
+        y = y + bias.to(COMPUTE)
     return F.silu(y) if post_silu else y
 
 
 def timestep_embedding(t, dim, flip_sin_to_cos=True, freq_shift=0.0):
     half = dim // 2
     freqs = torch.exp(-math.log(10000.0) * torch.arange(half, dtype=torch.float32) / (half - freq_shift))
-    arg = t.float()[:, None] * freqs[None]
+    arg = t.to(COMPUTE)[:, None] * freqs[None]
     emb = torch.cat([torch.sin(arg), torch.cos(arg)], -1)
     return torch.cat([emb[:, half:], emb[:, :half]], -1) if flip_sin_to_cos else emb
 
 
 def fourier_embed(x, num_freqs):
-    outs = [x.float()]
+    outs = [x.to(COMPUTE)]
     for k in range(num_freqs):
-        outs += [torch.sin(x.float() * 2.0 ** k), torch.cos(x.float() * 2.0 ** k)]
+        outs += [torch.sin(x.to(COMPUTE) * 2.0 ** k), torch.cos(x.to(COMPUTE) * 2.0 ** k)]
     return torch.cat(outs, -1)
 
 
 def nchw_to_nhwc(x):
     n, c, h, w = x.shape
-    return _act(x.float().permute(0, 2, 3, 1).reshape(n * h * w, c))
+    return _act(x.to(COMPUTE).permute(0, 2, 3, 1).reshape(n * h * w, c))
 
 
 def nhwc_to_nchw(x, n, c, h, w, dtype=torch.float32):
-    return x.float().reshape(n, h, w, -1)[..., :c].permute(0, 3, 1, 2).contiguous().to(dtype)
+    return x.to(COMPUTE).reshape(n, h, w, -1)[..., :c].permute(0, 3, 1, 2).contiguous().to(dtype)
 
 
 def f32_to_bf16(x):
@@ -306,11 +324,11 @@ def f32_to_bf16(x):
 
 
 def pack_latents(x, cpad=64, repeat=1):
-    return _act(F.pad(x.float(), (0, cpad - x.shape[1]))).repeat(repeat, 1)
+    return _act(F.pad(x.to(COMPUTE), (0, cpad - x.shape[1]))).repeat(repeat, 1)
 
 
 def _cfg_combine(eps, cfg, guidance, c, npix):
-    e = eps[:, :c].float()
+    e = eps[:, :c].to(COMPUTE)
     return e[:npix] + guidance * (e[npix:] - e[:npix]) if cfg else e
 
 

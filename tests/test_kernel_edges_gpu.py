@@ -4,8 +4,9 @@ kernel, the direct convolution and the adaptive pool.
 
 The GEMM, attention and GroupNorm kernels have f16 twins (the denoising step of a model with fp16 parameters) that share
 their bodies through Act<F16> (csrc/ptx.cuh); those tests take the element type `dt` (bf16 | f16, `with_dt`) and run both at
-the same edges, the f16 cases under ids that start with "f16-".  The VAE launches, the direct convolution and the adaptive
-pool are bf16 / fp32 only.
+the same edges, the f16 cases under ids that start with "f16-".  The VAE decoder's GEMM launches run in both types too (an
+fp16 VAE computes in f16); the direct convolution and the adaptive pool are bf16 / fp32 here (the f16 direct convolution is
+test_vae_fp16_gpu.py's).
 
 Every reference is computed in float64 on the GPU from the same bf16- (or f16-) rounded inputs.  Every output is written
 into a larger buffer pre-filled with a NaN bit pattern: at least one full 128-row M tile of guard rows before and after the
@@ -53,16 +54,17 @@ def _randn(*shape, g, scale=1.0):
 class Guarded:
     """A [rows, cols] output at column `col0` of a [G + rows + G, ld] buffer filled with a NaN bit pattern."""
 
-    def __init__(self, rows, cols, dtype=BF16, ld=None, col0=0):
+    def __init__(self, rows, cols, dtype=BF16, ld=None, col0=0, device="cuda"):
         self.rows, self.cols, self.col0, self.ld = rows, cols, col0, ld or cols
         assert col0 + cols <= self.ld
         self.itype, self.fill = _FILL[dtype]
-        self.buf = torch.empty((rows + 2 * G, self.ld), dtype=dtype, device="cuda")
+        self.buf = torch.empty((rows + 2 * G, self.ld), dtype=dtype, device=device)
         self.buf.view(self.itype).fill_(self.fill)
         self.out = self.buf[G:G + rows, col0:col0 + cols]
 
     def check(self, what=""):
-        torch.cuda.synchronize()
+        if self.buf.is_cuda:
+            torch.cuda.synchronize()
         bits = self.buf.view(self.itype)
         outside = torch.ones_like(bits, dtype=torch.bool)
         outside[G:G + self.rows, self.col0:self.col0 + self.cols] = False
@@ -73,11 +75,28 @@ class Guarded:
         assert left == 0, f"{what}: {left} output elements never written"
 
 
+def _tol_bf16(ref, ref_max=None):
+    """_close_bf16's elementwise tolerance for a float64 reference; ref_max = max |ref| over the whole output (default: over
+    `ref`), so that an output checked in pieces is held to the tolerance of the whole."""
+    return ref.abs() * 2.0 ** -7 + 2e-3 * (ref.abs().max() if ref_max is None else ref_max)
+
+
+def _tol_f16(ref, ref_max=None):
+    """_close_f16's elementwise tolerance: one f16 ulp of ref plus 1e-4 of max |ref| (ref_max as in _tol_bf16)."""
+    ulp = torch.exp2(torch.floor(torch.log2(ref.abs().clamp_min(2.0 ** -14))) - 10)
+    return ulp + 1e-4 * (ref.abs().max() if ref_max is None else ref_max)
+
+
+def _tol_f32(ref, ref_max=None):
+    """_close_f32's tolerance, one value for every element: 3e-5 of max |ref| (ref_max as in _tol_bf16)."""
+    return 3e-5 * (ref.abs().max() if ref_max is None else ref_max)
+
+
 def _close_bf16(out, ref, what=""):
     """Every element within one bf16 rounding step of the reference plus accumulation-order slack (test_gemm_pair_gpu.py)."""
     ref = ref.to(F64)
     err = (out.to(F64) - ref).abs()
-    tol = ref.abs() * 2.0 ** -7 + 2e-3 * ref.abs().max()
+    tol = _tol_bf16(ref)
     bad = (err > tol).nonzero()
     assert bad.shape[0] == 0, f"{what}: {bad.shape[0]} elements off, first at {tuple(bad[0].tolist())}, " \
                               f"max err {err.max().item():.3e} (max |ref| {ref.abs().max().item():.3e})"
@@ -89,8 +108,7 @@ def _close_f16(out, ref, what=""):
     csrc/ptx.cuh), so a store at any coarser precision (bf16's 8 bits) fails it."""
     ref = ref.to(F64)
     err = (out.to(F64) - ref).abs()
-    ulp = torch.exp2(torch.floor(torch.log2(ref.abs().clamp_min(2.0 ** -14))) - 10)
-    tol = ulp + 1e-4 * ref.abs().max()
+    tol = _tol_f16(ref)
     bad = (err > tol).nonzero()
     assert bad.shape[0] == 0, f"{what}: {bad.shape[0]} elements off, first at {tuple(bad[0].tolist())}, " \
                               f"max err {err.max().item():.3e} (max |ref| {ref.abs().max().item():.3e})"
@@ -99,7 +117,7 @@ def _close_f16(out, ref, what=""):
 def _close_f32(out, ref, what=""):
     ref = ref.to(F64)
     err = (out.to(F64) - ref).abs()
-    tol = 3e-5 * ref.abs().max()
+    tol = _tol_f32(ref)
     bad = (err > tol).nonzero()
     assert bad.shape[0] == 0, f"{what}: {bad.shape[0]} elements off, first at {tuple(bad[0].tolist())}, " \
                               f"max err {err.max().item():.3e} (tolerance {tol.item():.3e})"
@@ -184,8 +202,10 @@ PRODUCT_CONVS = {
     "vae_shortcut_224x400": (1, 224, 400, 256, 128, 1, 1, 0, {}),
     "downsample_s2": (12, 28, 50, 320, 320, 3, 2, 1, {}),
 }
-# the UNet / ControlNet launches in both element types; the VAE decoder is bf16 whatever its parameters (INTEGRATION.md)
-PRODUCT_F16 = ("conv_in", "conv_out", "downsample_s2")
+# all of them in both element types: the UNet / ControlNet, and the VAE decoder, which computes in f16 when its parameters
+# are fp16 (AutoencoderKL.engine)
+PRODUCT_F16 = ("conv_in", "conv_out", "vae_conv_out", "vae_mid_conv", "vae_up_56x100", "vae_conv1_112x200",
+               "vae_shortcut_112x200", "vae_conv2_224x400", "vae_shortcut_224x400", "downsample_s2")
 
 
 @pytest.mark.parametrize("variant", VARIANTS, ids=VARIANT_IDS)
@@ -198,34 +218,35 @@ def test_gemm_product_convs(cuda_lib, dt, case, variant):
     _close(out.out, ref, case)
 
 
-@pytest.mark.parametrize("variant", VARIANTS, ids=VARIANT_IDS)
-def test_gemm_vae_attention(cuda_lib, variant):
+@pytest.mark.parametrize("dt,variant", with_dt(VARIANTS, ids=VARIANT_IDS))
+def test_gemm_vae_attention(cuda_lib, dt, variant):
     """The three GEMMs of the VAE mid-block attention (engine.py VaeDecoderEngine._attention) for the second of two
-    28x50 images: S = q k^T (fp32, n_out = ldo = lp), V^T = W_v X^T (n_out = lp) and O = P V + b_v (K = lp)."""
+    28x50 images: S = q k^T (fp32, n_out = ldo = lp), V^T = W_v X^T (n_out = lp) and O = P V + b_v (K = lp), in both
+    element types (an fp16 VAE runs them in f16)."""
     g = _gen(2)
     n, L, C = 2, 1400, 512
     lp = (L + 63) // 64 * 64
     i = 1
-    q = _bf(_randn(n * L, C, g=g))
-    kbuf = torch.zeros(n * L + lp - L, C, dtype=BF16, device="cuda")
-    kbuf[: n * L] = _bf(_randn(n * L, C, g=g))
+    q = _randn(n * L, C, g=g).to(dt)
+    kbuf = torch.zeros(n * L + lp - L, C, dtype=dt, device="cuda")
+    kbuf[: n * L] = _randn(n * L, C, g=g).to(dt)
     s = Guarded(L, lp, F32)
     ops.linear(q[i * L:(i + 1) * L], kbuf[i * L: i * L + lp], out_f32=True, out_scale=C ** -0.5, out=s.out, ldo=lp,
                kernel_variant=variant)
     s.check("scores")
     _close_f32(s.out, (q[i * L:(i + 1) * L].to(F64) @ kbuf[i * L: i * L + lp].to(F64).t()) * C ** -0.5, "scores")
-    wv = _bf(_randn(C, C, g=g, scale=C ** -0.5))
-    t = _bf(_randn(n * L + lp - L, C, g=g))
-    vt = Guarded(C, lp)
+    wv = _randn(C, C, g=g, scale=C ** -0.5).to(dt)
+    t = _randn(n * L + lp - L, C, g=g).to(dt)
+    vt = Guarded(C, lp, dt)
     ops.linear(wv, t[i * L: i * L + lp], out=vt.out, ldo=lp, kernel_variant=variant)
     vt.check("V^T")
-    _close_bf16(vt.out, wv.to(F64) @ t[i * L: i * L + lp].to(F64).t(), "V^T")
-    p = _bf(torch.softmax(_randn(L, lp, g=g, scale=3.0), -1))
+    _close(vt.out, wv.to(F64) @ t[i * L: i * L + lp].to(F64).t(), "V^T")
+    p = torch.softmax(_randn(L, lp, g=g, scale=3.0), -1).to(dt)
     bv = _randn(C, g=g)
-    o = Guarded(L, C)
+    o = Guarded(L, C, dt)
     ops.linear(p, vt.out, bias=bv, out=o.out, ldo=C, kernel_variant=variant)
     o.check("P V")
-    _close_bf16(o.out, p.to(F64) @ vt.out.to(F64).t() + bv.to(F64), "P V")
+    _close(o.out, p.to(F64) @ vt.out.to(F64).t() + bv.to(F64), "P V")
 
 
 # (n, h, w, taps, stride): pixel counts 128k - 1, 128k + 1 and < 128, and last tiles that span several images
