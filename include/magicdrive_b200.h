@@ -391,6 +391,40 @@ int mdb_draw_box_edges_aa(const void* images, int images_is_f32, int n_images, i
                           const int* colors, const int* counts, const int* status, int capacity,
                           const unsigned char* palette, int n_colors, int transparent_bg, void* out, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Map images and view mosaics (magicdrive/misc/test_utils.py:258-321 run_one_batch; runner/map_visualizer.py:106-211
+ * render_static, render_dynamic, visualize_map; runner/img_utils.py:5-40 concat_6_views, img_m11_to_01): the pixels of
+ * the reference's `{n}_map.png`, `{n}_ori.png` and view mosaics, byte for byte.
+ * mdb_render_bev_map: maps [n_maps, channels, h, w], fp32 or (maps_is_f32 = 0) uint8 / bool, every value 0 or 1; pixel
+ *   (y, x) of map m is coloured from maps[m, :, y, x].  Channels [0, n_static) are the static layers, coloured as the
+ *   active class with the highest priority[c] (the first such channel on ties); channels [n_static, n_static + n_dynamic)
+ *   the dynamic layers, coloured as the first one set.  out: uint8 [n_maps, h, w, 3], dynamic over static over
+ *   (200, 200, 200).  colors: uint8 [n_static + n_dynamic, 4], RGB and 1 where the class has a colour; a static class
+ *   without a STATIC_PRIORITY rank has priority -1.  info: int64 [n_maps, 4] = {class mask of semantic_used: every active
+ *   static class, and with n_dynamic > 0 the dynamic argmax of every pixel (channel n_static where none is set); status,
+ *   bit 0 set when a value is neither 0 nor 1; the smallest (pixel << 6 | class), pixel = y * w + x, where an active
+ *   static class has priority -1 (the first such channel of the pixel); the smallest (pixel << 6 | class) where the
+ *   static class chosen at a pixel (under a dynamic layer or not) has colour flag 0}; an error word is all ones when the
+ *   error never arises.  n_static + n_dynamic in 1..64, <= channels; h, w <= 32767.
+ * mdb_place_map_u8: resized uint8 [n_maps, s, s, 3] -> per map m, Image.rotate(90) of it (np.rot90) with a legend pasted
+ *   to its right or below it.  desc: int64 [n_maps, 5] = {legend address (uint8 [lh, lw, 3]), lh, lw, 1 = right (lh == s:
+ *   image s x (s + lw)) or 0 = below (lw == s: image (s + lh) x s), byte offset of the image in out}.  max_pixels: the
+ *   largest image's pixel count.
+ * mdb_concat_views_u8: views uint8 [n_scenes, n_views, h, w, c], c = 3 or 4 -> out [n_scenes, 2h, max(3, n_views - 3) w,
+ *   c], views 0..2 on the first row and 3.. on the second (n_views >= 5), or with oneline [n_scenes, h, n_views w, c]
+ *   (n_views >= 2).  Uncovered pixels are black, alpha 255.
+ * mdb_m11_to_u8: x fp32 [n, 3, h, w] in [-1, 1] -> out uint8 [n, h, w, 3], ((x * 0.5 + 0.5) * 255) with each operation
+ *   rounded to fp32, truncated toward zero.
+ * ------------------------------------------------------------------------------------------------ */
+int mdb_render_bev_map(const void* maps, int maps_is_f32, int n_maps, int channels, int h, int w, int n_static,
+                       int n_dynamic, const int* priority, const unsigned char* colors, unsigned char* out, long long* info,
+                       void* stream);
+int mdb_place_map_u8(const unsigned char* resized, int n_maps, int s, const long long* desc, long long max_pixels,
+                     unsigned char* out, void* stream);
+int mdb_concat_views_u8(const unsigned char* views, int n_scenes, int n_views, int h, int w, int c, int oneline,
+                        unsigned char* out, void* stream);
+int mdb_m11_to_u8(const float* x, int n, int h, int w, unsigned char* out, void* stream);
+
 /* Barrier between the `world` GPUs of a sharding group over NVLink peer memory, as one stream operation (graph-capturable).
  * flag_ptrs_dev: device array of `world` pointers, entry i = GPU i's symmetric uint32[n_channels * world] flag array as mapped
  * into THIS GPU's address space; epoch_dev: this GPU's uint32[n_channels] counter; timed_out_dev: int set to 1 if a peer did

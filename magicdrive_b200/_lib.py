@@ -92,6 +92,10 @@ SIGNATURES = {
     "mdb_jpeg_encode_u8": (_i, [_vp, _i, _i, _i, _i, _vp, _ll, _vp, _ll, _vp, _vp]),
     "mdb_project_boxes": (_i, [_vp, _i, _vp, _vp, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "mdb_draw_box_edges_aa": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _vp, _vp]),
+    "mdb_render_bev_map": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "mdb_place_map_u8": (_i, [_vp, _i, _i, _vp, _ll, _vp, _vp]),
+    "mdb_concat_views_u8": (_i, [_vp, _i, _i, _i, _i, _i, _i, _vp, _vp]),
+    "mdb_m11_to_u8": (_i, [_vp, _i, _i, _i, _vp, _vp]),
 }
 
 
